@@ -60,7 +60,7 @@ def parse():
     p.add_argument("--verify-seconds", type=float, default=45.0, help="time budget of --verify")
     p.add_argument("--g-steps", type=int, default=5, help="timed generator-mode passes (0 = skip)")
     p.add_argument("--pairs", type=int, default=1 << 22, help="--phase reward: pairs per launch")
-    p.add_argument("--bfs-roots", type=int, default=1184, help="--phase bfs: roots per launch (8 per SM)")
+    p.add_argument("--bfs-roots", type=int, default=1056, help="--phase bfs: roots per launch (8 per SM of an H100 SXM)")
     p.add_argument("--score-mode", default="lazy", choices=["lazy", "literal"],
                    help="--impl reference: 'literal' recomputes the whole N x N all_score per root exactly as graph_gan.py:238 does "
                         "(only feasible at C1); 'lazy' scores the candidates on demand (the only form that exists at N >= 1e5)")
@@ -70,6 +70,8 @@ def parse():
                    help="K3 sweep: cp.async.bulk (TMA) pipeline or the per-thread-load kernel (A/B; sets GG_ADAM_PATH)")
     p.add_argument("--phase", default="sample", choices=["sample", "reward", "adam", "bfs", "update"],
                    help="what to time: the D-sampling pass (the BASELINE metric) or one of the other kernels of the path")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="--phase sample: write what the last timed pass returned to DIR/<name>.npy (float64)")
     return p.parse_args()
 
 
@@ -83,8 +85,15 @@ def make_inputs(args, rank):
         roots = np.flatnonzero(hg.degrees() > 0).astype(np.int32)
         args.roots = len(roots)
         return hg, np.asarray(c.emb_g, np.float64).astype(np.float32), roots, d
-    cache = "/tmp/gg_bench_cache/%s_seed%d.npz" % (args.workload, args.seed)
-    try:       # the CSR arrays of an earlier process on this box (the reference arm, another rank, an ncu pass)
+    # keyed by the sources that generate and arrange the graph, so that a cache written by other code is never read
+    import hashlib
+    import tempfile
+    src = hashlib.sha256()
+    for m in (synth, G):
+        with open(m.__file__, "rb") as f:
+            src.update(f.read())
+    cache = os.path.join(tempfile.gettempdir(), "gg_bench_cache", "%s_seed%d_%s.npz" % (args.workload, args.seed, src.hexdigest()[:16]))
+    try:       # the CSR arrays of an earlier process on this machine (the reference arm, another rank, a profiler pass)
         z = np.load(cache)
         hg = G.HostGraph.from_arrays(n, z["raw_indptr"], z["raw_adj"], z["indptr"], z["adj"])
     except (OSError, ValueError, KeyError, AssertionError):
@@ -117,7 +126,13 @@ class ClockSampler:
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
     def __init__(self, index):
-        self.rows, self.proc = [], None
+        self.rows, self.proc, self.gpu = [], None, {"name": None, "power_limit_w": None}
+        try:      # the card and its power limit are part of every number measured on it
+            f = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                               stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip().split(",")
+            self.gpu = {"name": f[0].strip(), "power_limit_w": float(f[1])}
+        except (OSError, subprocess.SubprocessError, IndexError, ValueError):
+            pass
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(index), "--query-gpu=" + self.Q,
                                           "--format=csv,noheader,nounits", "-lms", "100"],
@@ -139,7 +154,7 @@ class ClockSampler:
 
     def stop(self, t0, t1):
         if self.proc is None:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"], "gpu": self.gpu}
         time.sleep(0.15)
         self.proc.terminate()
         sm, smax, reasons = [], None, set()
@@ -158,7 +173,7 @@ class ClockSampler:
                 if v.lower().startswith("active"):
                     reasons.add(name)
         return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": smax, "reasons": sorted(reasons),
-                "samples": len(sm)}
+                "samples": len(sm), "gpu": self.gpu}
 
 
 # ----------------------------------------------------------------------------- CPU legs (oracle; checker only)
@@ -350,11 +365,11 @@ def workload_config(args, hg, d):
                         "(sample_num = deg(root), Philox RNG, update_ratio=1)" % (gen, n, deg, d, args.roots),
             "nnz": int(hg.adj.shape[0]), "max_deg": int(hg.max_deg),
             "l2_policy": "inputs larger than L2 (embedding matrix %d MB, tree rows %d MB)" % (
-                n * d * 4 >> 20, args.roots * (int(hg.adj.shape[0]) // 8) >> 20),
+                n * d * 4 // 10**6, args.roots * (int(hg.adj.shape[0]) // 8) // 10**6),
             "parallelism": "roots sharded over %d GPU(s), replicated graph+embeddings" % args.gpus}
 
 
-# ----------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------- CUDA arm
 def _peak():
     try:
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
@@ -362,7 +377,7 @@ def _peak():
             return float(peaks["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except (OSError, ValueError):
         pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s; not a measured peak)"
 
 
 def _ncu_traffic(kernel, key):
@@ -422,6 +437,30 @@ def _verify(args, hg, emb_h, roots, trees, out, smp, dev, seed, tag):
             "oracle": "oracle/gg_oracle.c (T1): ggo_bfs_parent + ggo_walk_pass on the roots of the last timed pass"}
 
 
+# elements per dumped array (6 MiB in float64).  A dump holds at most 9 arrays (6 outputs + 3 sample indices), so it
+# stays below 54 MiB; at the default workload (635 k rows, 322 k walks) nothing is sampled.
+DUMP_CAP = 3 << 18
+
+
+def dump_outputs(path, out):
+    """What the timed D pass hands its caller, as float64 DIR/<name>.npy: prepare_data_for_d's rows (center, neighbor,
+    label), every walk's sampled node and status, and the per-root accept flags.  An array longer than DUMP_CAP is
+    replaced by a fixed seeded sample of its positions, stored beside it as <group>_index.npy."""
+    os.makedirs(path, exist_ok=True)
+    center, neighbor, label = out.plan.rows
+    groups = {"rows": (int(out.plan.n_rows.item()), {"center": center, "neighbor": neighbor, "label": label}),
+              "walks": (int(out.n_walks), {"samples": out.samples, "status": out.status}),
+              "roots": (int(out.n_roots), {"root_ok": out.root_ok})}
+    for group, (n, arrays) in groups.items():
+        idx = None
+        if n > DUMP_CAP:
+            idx = np.sort(np.random.default_rng(12345).choice(n, DUMP_CAP, replace=False))
+            np.save(os.path.join(path, group + "_index.npy"), idx.astype(np.float64))
+        for name, t in arrays.items():
+            a = t[:n].cpu().numpy()
+            np.save(os.path.join(path, name + ".npy"), (a if idx is None else a[idx]).astype(np.float64))
+
+
 def smp_ld(emb_h):
     d = int(emb_h.shape[1])
     ld = 32
@@ -452,7 +491,7 @@ def run_b200(args):
     bias = torch.zeros(hg.n_node, dtype=torch.float32, device=dev)
     ev = lambda: torch.cuda.Event(enable_timing=True)
     # ---- tree construction (outside the metric: "trees resident", SURVEY 8d) -- timed on the device, reported
-    smp.build_trees(roots[:min(len(roots), 296)])                     # warm-up (allocates the builder's scratch)
+    smp.build_trees(roots[:min(len(roots), 264)])                     # warm-up (allocates the builder's scratch)
     torch.cuda.synchronize()
     e0, e1 = ev(), ev()
     e0.record()
@@ -535,6 +574,8 @@ def run_b200(args):
     clocks.wait_first()
     ms, cnts, t_start, t_end, last_out = timed(False)
     clk = clocks.stop(t_start, t_end)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_out)          # before later passes reuse the plan's buffers
     parity = None
     if rank == 0 and args.verify > 0:
         parity = _verify(args, hg, emb_h, roots, trees, last_out, smp, dev, args.seed, 2000 + args.steps - 1)
@@ -684,7 +725,8 @@ def run_b200(args):
             torch.cuda.synchronize()
             line["cpu_baseline"]["gpu_same_roots"] = {
                 "value": osub.counters_host()["accepted"] / (s0.elapsed_time(s1) / 5 * 1e-3), "unit": "neg_edges/s",
-                "note": "this GPU on exactly the cpu_baseline's root sample (%d roots: too few walks to fill 148 SMs)" % len(ref.sample)}
+                "note": "this GPU on exactly the cpu_baseline's root sample (%d roots: too few walks to fill %d SMs)" % (
+                    len(ref.sample), torch.cuda.get_device_properties(dev).multi_processor_count)}
             ref.close()
         emit(line)
     if world > 1:
@@ -877,6 +919,10 @@ def main():
     except OSError:
         _RESULT_FD = None
     os.environ["GG_ADAM_PATH"] = args.adam_path
+    if args.dump_outputs and (args.impl != "b200" or args.phase != "sample"):
+        sys.exit("--dump-outputs writes the outputs of the CUDA D-sampling pass (--impl b200 --phase sample)")
+    if args.dump_outputs and args.steps < 1:
+        sys.exit("--dump-outputs writes the last timed step's outputs: it needs --steps >= 1")
     if args.impl == "reference":
         return run_reference(args)
     if args.phase != "sample":

@@ -1,4 +1,4 @@
-"""graphgan_b200 -- B200 (sm_100a) implementation of GraphGAN's scoring-and-sampling hot path.
+"""graphgan_b200 -- H100 (sm_90a) implementation of GraphGAN's scoring-and-sampling hot path.
 
 Scope (SURVEY.md section 8): the graph-softmax walk sampler, BFS-tree construction, pairwise
 discriminator/generator scoring, reward, sparse gradients and the TF1-style Adam update, behind

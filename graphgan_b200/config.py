@@ -1,9 +1,9 @@
 """Run-time configuration: the reference's ``config`` surface, name for name and default for default.
 
 The reference keeps its hyper-parameters as attributes of a flat module that every layer reads at CALL
-time (``config.<name>``; /root/reference src/GraphGAN/config.py:1-41), so callers and tests can patch
+time (``config.<name>``; reference src/GraphGAN/config.py:1-41), so callers and tests can patch
 them.  This module is that flat module: the same names with the same values (they are the API), followed
-by the B200-only knobs, whose defaults leave the reference behaviour unchanged.
+by the knobs of this implementation, whose defaults leave the reference behaviour unchanged.
 ``src/GraphGAN/config.py`` aliases this module so ``import config`` keeps working from that directory.
 """
 
@@ -47,7 +47,7 @@ result_filename = _results + ".txt"
 cache_filename = "../../cache/" + dataset + ".pkl"      # unused here: trees are rebuilt on the GPU
 model_log = "../../log/"
 
-# ---- B200 additions (not in the reference)
+# ---- additions of this implementation (not in the reference)
 device = "cuda:0"                   # one process per GPU; LOCAL_RANK overrides the index under torchrun
 seed = 0                            # Philox key of the walk sampler and seed of the batch shuffles
 root_batch = 4096                   # roots whose BFS tree rows are resident at once (nnz / 8 bytes each)

@@ -1,4 +1,4 @@
-// adam.cu -- K3: TF1.8 AdamOptimizer "sparse" apply, which is dense (sm_100a).
+// adam.cu -- K3: TF1.8 AdamOptimizer "sparse" apply, which is dense (sm_90a).
 //
 // generator.py:30-31 / discriminator.py:31-32 call tf.train.AdamOptimizer(lr).minimize(loss)
 // on variables whose gradients are IndexedSlices.  TF 1.8's _apply_sparse_shared does
@@ -28,7 +28,7 @@ __global__ void __launch_bounds__(256, 4) adam_kernel(long long n_node, int ld, 
     adam_rows<false, 2>(n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, grad_rows, grad_bias, row_slot, lr_t, b1, b2, eps);
 }
 
-// ---------------------------------------------------------------- the same sweep with TMA bulk copies (Blackwell)
+// ---------------------------------------------------------------- the same sweep with TMA bulk copies (sm_90+)
 // The sweep is a pure stream (24 * N * ld bytes per step), so it is fed by the copy engine instead of per-thread loads:
 // one elected thread issues cp.async.bulk (global -> shared, completion on an mbarrier) for a tile of E, m and v, all
 // 256 threads update the tile in shared memory (the identical per-element operation sequence as adam_rows), and one

@@ -28,7 +28,7 @@ int sm_count() {
         int dev = 0, n = 0;
         if (cudaGetDevice(&dev) != cudaSuccess ||
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-            n = 148;  // B200
+            n = 132;  // H100 SXM
         cached = n;
     }
     return cached;

@@ -1,4 +1,4 @@
-// bfs.cu -- BFS-tree construction for a batch of roots (sm_100a).
+// bfs.cu -- BFS-tree construction for a batch of roots (sm_90a).
 //
 // Replaces GraphGAN.construct_trees (reference src/GraphGAN/graph_gan.py:84-108).  The reference stores, per
 // root, a dict node -> [father, children...]: O(N) Python objects per root and O(N^2) overall, which cannot exist

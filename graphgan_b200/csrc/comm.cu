@@ -1,7 +1,7 @@
-// comm.cu -- the data-parallel optimizer step with its collective INSIDE the library (sm_100a + NCCL over NVLink).
+// comm.cu -- the data-parallel optimizer step with its collective INSIDE the library (sm_90a + NCCL over NVLink).
 //
-// BASELINE.json north_star: "partition the root set over the 8xB200 box with a single NCCL [collective] of the
-// embedding gradients per step over NVLink".  The reference has no collective at all; the call sites this replaces
+// Data parallelism: partition the root set over the GPUs of one NVLink box, with a single NCCL collective of the
+// embedding gradients per step.  The reference has no collective at all; the call sites this replaces
 // are the per-batch sess.run loops of graph_gan.py:149-157 / 168-176, run on N replicas.
 //
 //   every rank:  K2 on ITS slice of the mini-batch  ->  ONE ncclAllGather of the compact gradients

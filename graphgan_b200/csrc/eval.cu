@@ -1,4 +1,4 @@
-// eval.cu -- the end-of-epoch quality line and embedding dump on the device (sm_100a; SURVEY.md section 8 row f4).
+// eval.cu -- the end-of-epoch quality line and embedding dump on the device (sm_90a; SURVEY.md section 8 row f4).
 //
 // Reference: GraphGAN.write_embeddings_to_file (graph_gan.py:293-306) writes both embedding matrices as text and
 // GraphGAN.evaluation (:308-319) -> LinkPredictEval.eval_link_prediction (src/evaluation/link_prediction.py:19-38)

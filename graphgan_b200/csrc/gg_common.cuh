@@ -1,4 +1,4 @@
-// gg_common.cuh -- shared device helpers for libgraphgan_b200 (sm_100a).
+// gg_common.cuh -- shared device helpers for libgraphgan_b200 (sm_90a).
 //
 // Every arithmetic helper here executes the "canonical" operation sequence written down in
 // DESIGN.md section 3, with explicit round-to-nearest intrinsics so that nvcc can neither

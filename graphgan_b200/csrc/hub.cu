@@ -1,4 +1,4 @@
-// hub.cu -- per-pass precomputation that removes the walk's redundant work (sm_100a).
+// hub.cu -- per-pass precomputation that removes the walk's redundant work (sm_90a).
 //
 // The reference recomputes E.E^T + b for EVERY root (graph_gan.py:238) and re-derives the same
 // root-step softmax for each of the root's sample_num walks (:260-262).  Two exact reuses:

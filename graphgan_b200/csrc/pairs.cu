@@ -1,4 +1,4 @@
-// pairs.cu -- K2: pairwise scoring, reward, sparse gradients; window-pair expansion (sm_100a).
+// pairs.cu -- K2: pairwise scoring, reward, sparse gradients; window-pair expansion (sm_90a).
 //
 //   score_k = e[i_k] . e[j_k] + b[j_k]      discriminator.py:21-24 / generator.py:22-25
 //   reward  = log(1 + exp(clip(score,-10,10)))  discriminator.py:33-34 (fetched at graph_gan.py:220-222)

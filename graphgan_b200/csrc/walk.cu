@@ -1,4 +1,4 @@
-// walk.cu -- K1, the graph-softmax walk sampler (sm_100a).
+// walk.cu -- K1, the graph-softmax walk sampler (sm_90a).
 //
 // Replaces GraphGAN.sample (reference src/GraphGAN/graph_gan.py:225-270) for a whole batch of
 // roots: one warp owns one walk at a time (persistent CTAs pull walk ids from a global

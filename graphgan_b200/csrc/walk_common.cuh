@@ -8,18 +8,20 @@ namespace gg {
 
 // Tuning knobs (compile-time; tools/variants.py builds A/B libraries with -DGG_...): the walk kernels are latency
 // bound, so the trade is occupancy (registers, shared memory per warp) against loads in flight per warp (unrolling)
-// and against instruction footprint (the hot path must stay near the 32 KB L1.5 instruction cache).
+// and against instruction footprint (the hot path must stay near the 32 KB L1.5 instruction cache).  The defaults are
+// the H100's A/B winner (DESIGN.md section 8.1): 3 CTAs/SM at 80 registers, 2048 scores per warp in shared memory
+// (3 x 74 KB of the SM's 228 KB), 4 tiles in flight.
 #ifndef GG_SC_CAP
-#define GG_SC_CAP 1024
+#define GG_SC_CAP 2048
 #endif
 #ifndef GG_UNR
-#define GG_UNR 2
+#define GG_UNR 4
 #endif
 #ifndef GG_UNR_S1
 #define GG_UNR_S1 8
 #endif
 #ifndef GG_WALK_MIN_CTAS
-#define GG_WALK_MIN_CTAS 4
+#define GG_WALK_MIN_CTAS 3
 #endif
 constexpr int WARPS_PER_CTA = 8;
 constexpr int WALK_MIN_CTAS = GG_WALK_MIN_CTAS;   // CTAs per SM the walk kernels are compiled and launched for

@@ -1,5 +1,5 @@
 /*
- * graphgan_b200.h -- C ABI of libgraphgan_b200.so, the B200 (sm_100a) implementation of
+ * graphgan_b200.h -- C ABI of libgraphgan_b200.so, the H100 (sm_90a) implementation of
  * GraphGAN's scoring-and-sampling hot path.
  *
  * The reference (hwwang55/GraphGAN) has no native code and no FFI: its seam is the five

@@ -4,7 +4,7 @@
  * A plain-C, single-threaded restatement of GraphGAN's graph-softmax walk
  * (reference: src/GraphGAN/graph_gan.py:182-270, src/utils.py:131-133 and the legacy
  * numpy RandomState.choice inverse-CDF step called at graph_gan.py:262) with a FULLY
- * SPECIFIED arithmetic, so that the sm_100a kernels in graphgan_b200/csrc can execute
+ * SPECIFIED arithmetic, so that the sm_90a kernels in graphgan_b200/csrc can execute
  * the identical operation sequence and be compared bit-for-bit.
  *
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
@@ -13,7 +13,7 @@
  * Parity status: the reference's TF1.8 kernels cannot run here (no TensorFlow), so the
  * dense arithmetic (sgemm order, numpy SIMD exp) is "parity unpinned"; the control flow,
  * RNG consumption, candidate order and tree mutation ARE pinned against the reference's
- * own Python (tests/golden/make_golden.py imports it from /root/reference).
+ * own Python (tests/golden/make_golden.py imports it from a reference checkout).
  *
  * Canonical arithmetic (shared with the CUDA kernels, see DESIGN.md section 3):
  *   rows      : [N, ld] fp32, ld = round_up(d, 32), zero padded.

@@ -1,7 +1,7 @@
 """Drop-in for the reference's src/GraphGAN/config.py: same names, same defaults.
 
 Kept as a thin alias so that ``import config`` from the working directory src/GraphGAN (the
-reference's import style, graph_gan.py:8) resolves to the one configuration module the B200
+reference's import style, graph_gan.py:8) resolves to the one configuration module the CUDA
 implementation reads."""
 import os
 import sys

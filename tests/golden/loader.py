@@ -28,6 +28,10 @@ def _sha(*arrs):
 def load(name):
     z = np.load(os.path.join(HERE, name + ".npz"))
     c = Case({k: z[k] for k in z.files})
+    side = os.path.join(HERE, name + "_pretrain.npz")   # make_golden.py: the pretrain rows live in a file of their own
+    if os.path.exists(side):
+        p = np.load(side)
+        c.update({k: p[k] for k in p.files})
     n, d, seed = int(c["n_node"]), int(c["d"]), int(c["seed"])
     rs = np.random.RandomState(seed + 1000)
     if "pretrain_q1e6" in c:

@@ -1,15 +1,15 @@
 #!/usr/bin/env python
 """Generate the golden fixtures in tests/golden/ by running the UNMODIFIED reference.
 
-Run in the authoring container only (needs /root/reference; the GPU box has no copy):
+Needs a checkout of the reference (hwwang55/GraphGAN @ 3f1c3f7); the tests only read the fixtures it writes:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <path to the GraphGAN checkout>
 
 What runs: the reference's own host half -- ``GraphGAN.construct_trees``, ``sample``,
 ``prepare_data_for_d``, ``prepare_data_for_g``, ``get_node_pairs_from_path``
-(/root/reference/src/GraphGAN/graph_gan.py:84-108, 182-291) and ``utils.read_edges`` /
-``utils.softmax`` (/root/reference/src/utils.py:12-47, 131-133) -- imported from
-/root/reference, never copied.  TensorFlow 1.8 is not installable here, so a stub
+(src/GraphGAN/graph_gan.py:84-108, 182-291) and ``utils.read_edges`` /
+``utils.softmax`` (src/utils.py:12-47, 131-133) -- imported from the reference
+checkout, never copied.  TensorFlow 1.8 is not installable here, so a stub
 ``tensorflow`` module satisfies the import and a stub session answers the two fetches the
 sampling code makes (``generator.all_score`` = fp32 E.E^T + b, generator.py:21;
 ``discriminator.reward`` = log(1+exp(clip(score,-10,10))), discriminator.py:21-24,33-34)
@@ -27,7 +27,7 @@ import types
 
 import numpy as np
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else "GraphGAN"
 OUT = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -273,7 +273,11 @@ def run_case(gg_mod, ref_utils, name, train_edges, test_edges, d, seed, emb=None
         out["g_reward"] = np.asarray(reward[:4096], np.float32)
     if extra:
         out.update(extra)
+    # the pretrain embeddings (cagrqc) go to <name>_pretrain.npz, so that no fixture file exceeds 1 MB; loader.load merges them
+    side = {k: out.pop(k) for k in list(out) if k.startswith("pretrain_")}
     np.savez_compressed(os.path.join(OUT, name + ".npz"), **out)
+    if side:
+        np.savez_compressed(os.path.join(OUT, name + "_pretrain.npz"), **side)
     print("%-14s N=%d d=%d  D rows=%d (steps %d)  G paths=%d pairs=%d  mutated=%d  draws=%d" % (
         name, n_node, d, len(center), len(rec_d.chosen), len(all_paths), len(node_1), len(mutated), total_draws))
 

@@ -190,7 +190,7 @@ def test_bench_reference_arm_machinery():
 
 def test_bench_reference_arm_prints_one_json_line():
     """`bench.py --impl reference` (the arm the driver runs beside ours): exactly one line on stdout, valid JSON with
-    the contract's keys; runs on the host cores only (no GPU, nothing read from /root/reference)."""
+    the contract's keys; runs on the host cores only (no GPU, nothing read from the reference checkout)."""
     import json
     import subprocess
     import sys

@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""tools/sass_evidence.py -- which Blackwell / Hopper-class instructions the shipped library contains, per kernel.
+"""tools/sass_evidence.py -- which Hopper-class (sm_90a) instructions the shipped library contains, per kernel.
 
-    python tools/sass_evidence.py > profiles/r02_sass_tma.txt
+    python tools/sass_evidence.py
 
 Counts, in `cuobjdump -sass graphgan_b200/libgraphgan_b200.so`: UBLKCP (cp.async.bulk, the TMA engine's 1-D bulk copy),
 SYNCS.* (mbarrier init / arrive.expect_tx / try_wait), UTMALDG/UTMASTG (tensor-map TMA; none: the streams here are 1-D),
-UTC*MMA (tcgen05; none by design: there is no dense contraction on this path), plus the classic LDG.E.128 / ATOMS / REDG."""
+HGMMA (wgmma; none by design: there is no dense contraction on this path), plus the classic LDG.E.128 / ATOMS / REDG."""
 import collections
 import os
 import re
@@ -15,7 +15,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = os.path.join(ROOT, "graphgan_b200", "libgraphgan_b200.so")
 sass = subprocess.run(["cuobjdump", "-sass", lib], stdout=subprocess.PIPE, text=True, check=True).stdout
-pat = {"UBLKCP": r"\bUBLKCP", "SYNCS (mbarrier)": r"\bSYNCS", "UTMALDG/UTMASTG": r"\bUTMA(LDG|STG)", "UTC*MMA (tcgen05)": r"\bUTC\w*MMA",
+pat = {"UBLKCP": r"\bUBLKCP", "SYNCS (mbarrier)": r"\bSYNCS", "UTMALDG/UTMASTG": r"\bUTMA(LDG|STG)", "HGMMA (wgmma)": r"\bHGMMA",
        "LDG.E.128": r"\bLDG\.E\.128", "LDGSTS": r"\bLDGSTS", "ATOMS": r"\bATOMS", "REDG/ATOMG": r"\b(REDG|ATOMG)", "FENCE.VIEW.ASYNC": r"\bFENCE\.VIEW\.ASYNC"}
 per = collections.OrderedDict()
 name = None
@@ -35,7 +35,7 @@ for line in sass.splitlines():
             if re.search(p, line):
                 per[name][k] += 1
 cols = ["instructions"] + list(pat)
-print("# SASS evidence: %s (cuobjdump -sass), sm_100a" % os.path.relpath(lib, ROOT))
+print("# SASS evidence: %s (cuobjdump -sass), sm_90a" % os.path.relpath(lib, ROOT))
 print("| kernel | " + " | ".join(cols) + " |")
 print("|---|" + "---|" * len(cols))
 tot = collections.Counter()

@@ -14,11 +14,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 VARIANTS = {
-    "base": [],                                   # defaults of csrc/walk_common.cuh: 4 CTAs/SM, 1024 scores, UNR 2 / 4
-    "r1": ["GG_WALK_MIN_CTAS=3", "GG_SC_CAP=2048", "GG_UNR=4"],      # the round-1 configuration
+    "base": [],                                   # defaults of csrc/walk_common.cuh: 3 CTAs/SM, 2048 scores, UNR 4 / 8
+    "occ4": ["GG_WALK_MIN_CTAS=4", "GG_SC_CAP=1024", "GG_UNR=2"],    # 4 CTAs/SM at 64 registers
     "occ5": ["GG_WALK_MIN_CTAS=5"],
-    "unr1": ["GG_UNR=1"],
-    "s1unr8": ["GG_UNR_S1=8"],
+    "unr2": ["GG_UNR=2"],
 }
 
 
