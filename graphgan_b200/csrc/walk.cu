@@ -330,7 +330,14 @@ __global__ void root_step_kernel(const __grid_constant__ gg_walk_desc d) {
     atomicAdd(d.s1_cnt + o + idx, 1);
 }
 
-constexpr int S1_SINGLES = 8192, S1_CHUNK = 16;
+// Queue items that are one pair each.  The queue is sorted by decreasing child degree, and a chunk of S1_CHUNK pairs runs
+// on one warp, so the pairs must be short by the time chunks start: at C3 the 8192nd pair's child still has ~3 000
+// neighbours (a chunk there is ~16 such lists in series: the launch's tail), the 65 536th ~140.  Measured at C3 on the
+// H100: 8192 -> 1.01 ms for the depth-1 stage, 32768 and 65536 -> 0.83 ms (DESIGN.md section 8.1).
+#ifndef GG_S1_SINGLES
+#define GG_S1_SINGLES 65536
+#endif
+constexpr int S1_SINGLES = GG_S1_SINGLES, S1_CHUNK = 16;
 
 template <int CPL>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) step1_cdf_kernel(const __grid_constant__ gg_walk_desc d) {
