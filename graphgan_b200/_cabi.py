@@ -9,7 +9,7 @@ import os
 from . import _build
 
 _LIB = None
-ABI_VERSION = 3      # == GG_ABI_VERSION of include/graphgan_b200.h
+ABI_VERSION = 4      # == GG_ABI_VERSION of include/graphgan_b200.h
 
 
 class GGError(RuntimeError):
@@ -59,6 +59,8 @@ SIGNATURES = {
     "gg_pair_reward": (C.c_int, [_I64, _P, _P, _P, _P, _I32, _P, _P]),
     "gg_all_score": (C.c_int, [_I64, _P, _P, _I32, _P, _P]),
     "gg_pair_grad": (C.c_int, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P, _P, _P]),
+    "gg_pair_grad_scratch_bytes": (C.c_int, [_I32, _I32, C.POINTER(_I64)]),
+    "gg_pair_grad_ex": (C.c_int, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P, _P, _P, _I64, _I32, _P]),
     "gg_grad_buf_floats": (_I64, [_I32, _I32]),
     "gg_grad_merge": (C.c_int, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P]),
     "gg_comm_unique_id": (C.c_int, [_P]),
@@ -76,6 +78,8 @@ SIGNATURES = {
     "gg_adam_apply": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _F, _F, _F, _F, _P]),
     "gg_train_steps": (C.c_int, [_I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P,
                                 _F, _F, _F, _F, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
+    "gg_train_steps_ex": (C.c_int, [_I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P,
+                                   _F, _F, _F, _F, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, _I64, _P]),
     "gg_train_loop": (C.c_int, [_I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P,
                                _F, _F, _F, _F, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, _P]),
     "gg_train_fused": (C.c_int, [_I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _F,

@@ -7,8 +7,13 @@
 //
 // Gradients are produced in TF1.8's IndexedSlices form after _apply_sparse_duplicate_indices:
 // unique row ids + per-row sums (entries accumulated in (i-side 0..B-1, j-side 0..B-1) order,
-// deterministic).  A mini-batch is tiny (config.batch_size_* = 64), so one CTA does it; the
-// expensive part of a step is K3's dense sweep (adam.cu).  Gather-bound, fp32, no tensor cores.
+// deterministic).  The reference's mini-batch is small (config.batch_size_* = 64), so one CTA does
+// up to GG_MAX_BATCH = 1024 pairs here; the expensive part of such a step is K3's dense sweep
+// (adam.cu).  Larger batches go to the multi-CTA gradient of grad_multi.cu (gg_pair_grad_ex), which
+// computes the same bits: slots in first-occurrence order, and per slot one +0-started __fadd_rn
+// chain per coordinate over the slot's entries in entry order (bias: j-side entries only).  Such a
+// chain is serial, so the batch's longest slot is the floor of that path.  Gather-bound, fp32, no
+// tensor cores.
 #include "update_dev.cuh"
 
 namespace gg {

@@ -14,14 +14,27 @@ extern "C" int gg_train_steps(int32_t mode, int64_t n_rows, const int64_t *start
                               float lambda, int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias,
                               int32_t *row_slot, float lr, float beta1, float beta2, float eps, float *beta1_power,
                               float *beta2_power, void *stream) {
-    GG_REQUIRE(start_list && beta1_power && beta2_power, "null host pointer");
     GG_REQUIRE(batch_size > 0 && batch_size <= GG_MAX_BATCH, "batch size out of range");
+    return gg_train_steps_ex(mode, n_rows, start_list, n_starts, batch_size, node_id, node_neighbor_id, aux, n_node, ld, emb,
+                             m_emb, v_emb, bias, m_bias, v_bias, lambda, n_unique, uniq_ids, grad_rows, grad_bias, row_slot, lr,
+                             beta1, beta2, eps, beta1_power, beta2_power, nullptr, 0, stream);
+}
+
+extern "C" int gg_train_steps_ex(int32_t mode, int64_t n_rows, const int64_t *start_list, int64_t n_starts, int32_t batch_size,
+                                 const int32_t *node_id, const int32_t *node_neighbor_id, const float *aux, int64_t n_node,
+                                 int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias, float *m_bias, float *v_bias,
+                                 float lambda, int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias,
+                                 int32_t *row_slot, float lr, float beta1, float beta2, float eps, float *beta1_power,
+                                 float *beta2_power, void *scratch, int64_t scratch_bytes, void *stream) {
+    GG_REQUIRE(start_list && beta1_power && beta2_power, "null host pointer");
+    GG_REQUIRE(batch_size > 0, "batch size out of range");
     for (int64_t s = 0; s < n_starts; ++s) {
         const int64_t start = start_list[s];
         GG_REQUIRE(start >= 0 && start < n_rows, "start out of range");
         const int64_t end = start + batch_size < n_rows ? start + batch_size : n_rows;
-        int rc = gg_pair_grad(mode, (int32_t)(end - start), 0, node_id + start, node_neighbor_id + start, aux + start, emb, bias,
-                              ld, lambda, n_unique, uniq_ids, grad_rows, grad_bias, row_slot, stream);
+        int rc = gg_pair_grad_ex(mode, (int32_t)(end - start), 0, node_id + start, node_neighbor_id + start, aux + start, emb,
+                                 bias, ld, lambda, n_unique, uniq_ids, grad_rows, grad_bias, row_slot, scratch, scratch_bytes, 0,
+                                 stream);
         if (rc) return rc;
         // lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t), fp32 step by step like the TF graph (and model.py)
         volatile float one_m_b2 = 1.0f - *beta2_power;

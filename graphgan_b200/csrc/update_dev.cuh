@@ -27,6 +27,21 @@ __device__ __forceinline__ float group_dot_t(const float *a, const float *b, int
     return group8_sum(s);
 }
 
+// dL/dscore of the pair (i, j) with label / reward a_k, computed by the 8-lane group that holds it (lane g of the
+// group; every lane returns the same value): the canonical group dot, + bias[j], the sigmoid in fp64, the D or G
+// formula.  The one-CTA gradient (pair_lists) and the multi-CTA gradient (grad_multi.cu) both call it.
+template <bool COH>
+__device__ __forceinline__ float pair_delta(int mode, int batch_total, int i, int j, float a_k, const float *emb,
+                                            const float *bias, int ld, int g) {
+    const float bj = ldf<COH>(bias + j);
+    float s = group_dot_t<COH>(emb + (size_t)i * ld, emb + (size_t)j * ld, ld, g);
+    s = __fadd_rn(s, bj);
+    const float p = (float)(1.0 / (1.0 + exp(-(double)s)));   // sigmoid (B values: fp64 costs nothing)
+    if (mode == 0) return p - a_k;                              // d/ds sigmoid_xent(label, s) = sigmoid(s) - label
+    // d/ds [-(1/B) r log(clip(p,1e-5,1))] = -(r/B)(1-p) where the clip passes (p >= 1e-5)
+    return (p >= 1e-5f) ? -(a_k / (float)batch_total) * (1.0f - p) : 0.0f;
+}
+
 // Shared memory of one mini-batch gradient: ids, slot, rank, list (2B ints each), offsets (2B + 2), delta (B).
 __host__ __device__ inline size_t pair_grad_smem_bytes(int B) { return (size_t)(11 * B + 8) * 4; }
 
@@ -67,21 +82,9 @@ __device__ __forceinline__ int pair_lists(int *smem, int mode, int B, int batch_
         const int k = k0 + grp;
         const bool valid = k < B;
         const int i = valid ? ni[k] : 0, j = valid ? nj[k] : 0;
-        const float bj = ldf<COH>(bias + j);
         const float a_k = valid ? aux[k] : 0.0f;
-        float s = group_dot_t<COH>(emb + (size_t)i * ld, emb + (size_t)j * ld, ld, g);
-        if (valid && g == 0) {
-            s = __fadd_rn(s, bj);
-            const float p = (float)(1.0 / (1.0 + exp(-(double)s)));   // sigmoid (B values: fp64 costs nothing)
-            float d;
-            if (mode == 0) {
-                d = p - a_k;                             // d/ds sigmoid_xent(label, s) = sigmoid(s) - label
-            } else {
-                // d/ds [-(1/B) r log(clip(p,1e-5,1))] = -(r/B)(1-p) where the clip passes (p >= 1e-5)
-                d = (p >= 1e-5f) ? -(a_k / (float)batch_total) * (1.0f - p) : 0.0f;
-            }
-            delta[k] = d;
-        }
+        const float d = pair_delta<COH>(mode, batch_total, i, j, a_k, emb, bias, ld, g);
+        if (valid && g == 0) delta[k] = d;
     }
     __syncthreads();
     // ---- unique, phase A: 8 lanes per entry scan the earlier entries (strided) for equal ids

@@ -56,6 +56,7 @@ class PairModel:
         self.sync_words = torch.zeros(8, dtype=torch.int64, device=dev)     # flag, counter, cycle breakdown of gg_train_loop
         self.grad_rows = z(2 * MAX_BATCH, self.ld)
         self._emb2 = self._bias2 = None          # second parameter buffers of gg_train_fused (allocated on first use)
+        self._scratch = None                     # multi-CTA gradient scratch (batches above GG_MAX_BATCH; first use)
         self.grad_bias = z(2 * MAX_BATCH)
         # tf.train.AdamOptimizer defaults
         self.lr, self.lam = np.float32(lr), np.float32(lam)
@@ -91,9 +92,15 @@ class PairModel:
         B = int(i.shape[0])
         if B == 0:
             return
-        if B > MAX_BATCH:
-            raise ValueError("batch of %d pairs exceeds GG_MAX_BATCH=%d" % (B, MAX_BATCH))
         st = self._stream()
+        if B > MAX_BATCH:
+            scratch = self._large_batch_buffers(B)
+            _cabi.check(self.lib.gg_pair_grad_ex(self._step_mode, B, 0, ptr(i), ptr(j), ptr(a), ptr(self.emb), ptr(self.bias_t),
+                                                 self.ld, C.c_float(float(self.lam)), ptr(self.n_unique), ptr(self.uniq_ids),
+                                                 ptr(self.grad_rows), ptr(self.grad_bias), ptr(self.row_slot), ptr(scratch),
+                                                 scratch.numel(), 0, st), "gg_pair_grad_ex")
+            self.apply_adam()
+            return
         _cabi.check(self.lib.gg_pair_grad(self._step_mode, B, 0, ptr(i), ptr(j), ptr(a), ptr(self.emb), ptr(self.bias_t),
                                           self.ld, C.c_float(float(self.lam)), ptr(self.n_unique), ptr(self.uniq_ids),
                                           ptr(self.grad_rows), ptr(self.grad_bias), ptr(self.row_slot), st),
@@ -102,14 +109,29 @@ class PairModel:
 
     def train_steps(self, node_id, node_neighbor_id, aux, start_list, batch_size, persistent=None):
         """All optimizer steps of one inner epoch (graph_gan.py:149-157 / 168-176): ``start_list`` is the shuffled
-        list of batch starts; rows come from the device arrays.  Identical to calling ``step`` per batch."""
+        list of batch starts; rows come from the device arrays.  Identical to calling ``step`` per batch.  Batches above
+        GG_MAX_BATCH pairs run in the C loop (the persistent loops keep a one-CTA gradient)."""
+        if batch_size > MAX_BATCH and persistent:
+            raise ValueError("the persistent step loops take at most GG_MAX_BATCH=%d pairs per batch, not %d (use persistent=None)"
+                             % (MAX_BATCH, batch_size))
         i, j, a = self._dev_i32(node_id), self._dev_i32(node_neighbor_id), self._dev_f32(aux)
         starts = np.ascontiguousarray(np.asarray(start_list, np.int64))
         if starts.size == 0:
             return
-        if batch_size > MAX_BATCH:
-            raise ValueError("batch of %d pairs exceeds GG_MAX_BATCH=%d" % (batch_size, MAX_BATCH))
         b1p, b2p = C.c_float(float(self.beta1_power)), C.c_float(float(self.beta2_power))
+        if batch_size > MAX_BATCH:
+            scratch = self._large_batch_buffers(batch_size)
+            _cabi.check(self.lib.gg_train_steps_ex(self._step_mode, int(i.shape[0]), starts.ctypes.data_as(C.c_void_p),
+                                                   int(starts.size), int(batch_size), ptr(i), ptr(j), ptr(a), self.n_node, self.ld,
+                                                   ptr(self.emb), ptr(self.m_emb), ptr(self.v_emb), ptr(self.bias_t), ptr(self.m_bias),
+                                                   ptr(self.v_bias), C.c_float(float(self.lam)), ptr(self.n_unique), ptr(self.uniq_ids),
+                                                   ptr(self.grad_rows), ptr(self.grad_bias), ptr(self.row_slot), C.c_float(float(self.lr)),
+                                                   C.c_float(float(self.beta1)), C.c_float(float(self.beta2)), C.c_float(float(self.eps)),
+                                                   C.byref(b1p), C.byref(b2p), ptr(scratch), scratch.numel(), self._stream()),
+                        "gg_train_steps_ex")
+            self.beta1_power, self.beta2_power = np.float32(b1p.value), np.float32(b2p.value)
+            self.step_count += int(starts.size)
+            return
         if persistent is None:
             # the persistent loops win while the sweep is small (C1, 4 MB of E/m/v: 11.0 us/step fused, 13.9 two-barrier, 18.4
             # as two launches per step); from ~60 MB on the sweep is faster as its own full-occupancy launch (N = 40k,
@@ -148,6 +170,20 @@ class PairModel:
                                             C.byref(b1p), C.byref(b2p), self._stream()), "gg_train_steps")
         self.beta1_power, self.beta2_power = np.float32(b1p.value), np.float32(b2p.value)
         self.step_count += int(starts.size)
+
+    def _large_batch_buffers(self, B):
+        """Grow uniq_ids / grad_rows / grad_bias to 2B entries and the multi-CTA gradient's scratch to its size at B
+        (allocated on first use: models that never see a batch above GG_MAX_BATCH keep today's buffers)."""
+        torch = self.torch
+        if self.uniq_ids.numel() < 2 * B:
+            self.uniq_ids = torch.zeros(2 * B, dtype=torch.int32, device=self.device)
+            self.grad_rows = torch.zeros((2 * B, self.ld), dtype=torch.float32, device=self.device)
+            self.grad_bias = torch.zeros(2 * B, dtype=torch.float32, device=self.device)
+        n = C.c_int64(0)
+        _cabi.check(self.lib.gg_pair_grad_scratch_bytes(int(B), self.ld, C.byref(n)), "gg_pair_grad_scratch_bytes")
+        if self._scratch is None or self._scratch.numel() < n.value:
+            self._scratch = torch.empty(n.value, dtype=torch.uint8, device=self.device)   # caching allocator: 512-byte aligned
+        return self._scratch
 
     def apply_adam(self):
         st = self._stream()

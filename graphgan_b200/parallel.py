@@ -17,6 +17,7 @@ import numpy as np
 
 from . import _cabi
 from ._cabi import ptr
+from .model import MAX_BATCH
 
 
 def block_range(n, rank, world):
@@ -90,6 +91,12 @@ def connect_peer_memory(comm, capacity_floats, group=None):
     _cabi.check(lib.gg_comm_p2p_connect(comm, C.create_string_buffer(raw, 64 * world)), "gg_comm_p2p_connect")
 
 
+def _check_batch(B):
+    """The data-parallel gradient, exchange and merge are one-CTA kernels: refuse larger batches before communicating."""
+    if B > MAX_BATCH:
+        raise ValueError("data-parallel steps take at most GG_MAX_BATCH=%d pairs per batch, not %d" % (MAX_BATCH, B))
+
+
 class DataParallelStep:
     """Data-parallel replacement for PairModel.step / train_steps: same arguments (the WHOLE mini-batch, identical on
     every rank).  The step -- gradient of this rank's rows, ONE ncclAllGather of the compact gradients, rank-major merge,
@@ -139,6 +146,7 @@ class DataParallelStep:
         B = int(i.shape[0])
         if B == 0:
             return
+        _check_batch(B)
         cap = 2 * (-(-B // self.world))
         local, gathered = self._buffers(cap)
         self._select()
@@ -153,6 +161,7 @@ class DataParallelStep:
 
     def train_steps(self, node_id, node_neighbor_id, aux, start_list, batch_size):
         """All steps of one inner epoch (graph_gan.py:149-157 / 168-176) enqueued from C, one collective each."""
+        _check_batch(batch_size)
         m = self.model
         i, j, a = m._dev_i32(node_id), m._dev_i32(node_neighbor_id), m._dev_f32(aux)
         starts = np.ascontiguousarray(np.asarray(start_list, np.int64))

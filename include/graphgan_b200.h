@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 3
+#define GG_ABI_VERSION 4
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -223,6 +223,19 @@ int gg_pair_grad(int32_t mode, int32_t n_pairs, int32_t batch_total, const int32
                  const float *bias, int32_t ld, float lambda, int32_t *n_unique, int32_t *uniq_ids,
                  float *grad_rows, float *grad_bias, int32_t *row_slot, void *stream);
 
+/* The same gradient for any mini-batch size (1 .. 2^30 - 4096 pairs): outputs identical, bit for bit, to gg_pair_grad on
+ * every batch gg_pair_grad accepts, and the same in-order sums above GG_MAX_BATCH (csrc/grad_multi.cu).  Up to
+ * GG_MAX_BATCH pairs without flags it runs gg_pair_grad's one-CTA kernel; otherwise a multi-CTA path that needs
+ * `scratch` (device, 256-byte aligned, at least gg_pair_grad_scratch_bytes(n_pairs, ld) bytes).  uniq_ids, grad_rows
+ * and grad_bias hold 2 * n_pairs entries.  gg_pair_grad_scratch_bytes is a host-only size computation. */
+#define GG_GRAD_MULTI_CTA 1   /* flags: use the multi-CTA path even when n_pairs <= GG_MAX_BATCH (tests / A-B) */
+int gg_pair_grad_scratch_bytes(int32_t n_pairs, int32_t ld, int64_t *bytes);
+int gg_pair_grad_ex(int32_t mode, int32_t n_pairs, int32_t batch_total, const int32_t *node_id,
+                    const int32_t *node_neighbor_id, const float *aux, const float *emb, const float *bias,
+                    int32_t ld, float lambda, int32_t *n_unique, int32_t *uniq_ids, float *grad_rows,
+                    float *grad_bias, int32_t *row_slot, void *scratch, int64_t scratch_bytes,
+                    int32_t flags, void *stream);
+
 /* Data-parallel step: merge the compact gradients of `world` ranks (each laid out as one buffer of
  * gg_grad_buf_floats(cap, ld) floats: rows[cap, ld] | bias[cap] | ids[cap] (int32 bits) | n_unique) into
  * the final unique/summed form, rank-major entry order -- every rank computes the identical result
@@ -292,6 +305,14 @@ int gg_train_steps(int32_t mode, int64_t n_rows, const int64_t *start_list, int6
                    float *emb, float *m_emb, float *v_emb, float *bias, float *m_bias, float *v_bias, float lambda,
                    int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot, float lr,
                    float beta1, float beta2, float eps, float *beta1_power, float *beta2_power, void *stream);
+/* gg_train_steps for any batch size: gg_pair_grad_ex per step, with the caller's scratch (gg_pair_grad_scratch_bytes of
+ * batch_size; may be NULL when batch_size <= GG_MAX_BATCH).  uniq_ids / grad_rows / grad_bias hold 2 * batch_size entries. */
+int gg_train_steps_ex(int32_t mode, int64_t n_rows, const int64_t *start_list, int64_t n_starts, int32_t batch_size,
+                      const int32_t *node_id, const int32_t *node_neighbor_id, const float *aux, int64_t n_node,
+                      int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias, float *m_bias, float *v_bias,
+                      float lambda, int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias,
+                      int32_t *row_slot, float lr, float beta1, float beta2, float eps, float *beta1_power,
+                      float *beta2_power, void *scratch, int64_t scratch_bytes, void *stream);
 
 /* The same loop as gg_train_steps in ONE cooperative launch (persistent kernel; a ready flag and an arrival
  * counter order the gradient and the Adam sweep of every step).  start_list_dev is a DEVICE array; sync_words
