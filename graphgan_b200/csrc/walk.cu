@@ -415,13 +415,34 @@ struct FlatView {
     int *hub;              // [W] per level: items (indices into the level's list) that stand on a score-cached node
     int *item_n;           // [W] per item: candidate-list length | father flag << 30 (0: nothing left to do for the item)
     int *pool_ids;         // [W * stride] per item: its candidate ids
-    unsigned *ctr;         // counters: [0] tail length; level s: [1 + 4 s + {0: items, 1: hub items, 2: -, 3: work queue}]
+    unsigned *ctr;         // counters: [0] tail length; level s: [1 + 4 s + {0: items, 1: hub items, 2: distinct keys of a
+                           //     shared level, 3: work queue}]
     int stride;            // pool entries per item (>= hub_threshold: a node below the threshold has fewer neighbours)
     int steps;             // level-synchronous steps 1 .. steps
+    // shared levels (SHARE_LEVELS): one candidate list + CDF per distinct (root slot, node), every walk on it draws from it
+    unsigned long long *keys;   // [tbl_mask + 1] open-addressing table of slot * n_node + node (empty: ~0)
+    int *owner;            // [tbl_mask + 1] per table slot: the record that inserted the key (its item owns the list)
+    int *rec_slot;         // [W] per record: its table slot (-1: a hub item, run per walk)
+    int *uniq;             // [W] the level's distinct keys that are not score-cached, as the records that own them
+    double *pool_cdf;      // [W * (stride + 1)] per owning item: its un-normalised CDF and the total (cdf_store_raw)
+    unsigned long long tbl_mask;
 };
 constexpr int FLAT_MAX_STEPS = 14;
 constexpr int FLAT_CTR_WORDS = 1 + 4 * (FLAT_MAX_STEPS + 2);
 #define GG_FCTR(fv, s, k) ((fv).ctr + 1 + 4 * (s) + (k))
+// the record list of level s (a select: a run-time index into the kernel parameter would copy it to local memory)
+__device__ __forceinline__ int4 *level_list(const FlatView &fv, int s) { return (s & 1) ? fv.list[1] : fv.list[0]; }
+
+// Levels whose walks share one candidate list per distinct (root slot, node): bit s = level s, s >= 2 only (from step 2 on
+// the list is [tree father] + children(node) and depends on nothing else of the walk; step 1 is the depth-1 reuse).
+// 0 = no sharing: every level runs flat_enum + flat_choose per walk.
+#ifndef GG_SHARE_LEVELS
+#define GG_SHARE_LEVELS 0x4
+#endif
+constexpr unsigned SHARE_LEVELS = (unsigned)(GG_SHARE_LEVELS) & ~3u;
+__host__ __device__ constexpr bool level_shared(int s) { return s < 32 && ((SHARE_LEVELS >> s) & 1u); }
+// does any of the levels 1 .. steps share?
+inline bool any_level_shared(int steps) { return steps >= 2 && (SHARE_LEVELS & ((steps >= 31 ? ~0u : ((2u << steps) - 1u)))) != 0; }
 
 template <int CPL>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) walk_kernel(const __grid_constant__ gg_walk_desc d,
@@ -531,9 +552,9 @@ __device__ __forceinline__ bool step_includes_father(const gg_walk_desc &d, int 
     return true;
 }
 
-// lane 0: the walk made its choice at step s over n candidates
-__device__ __forceinline__ void flat_advance(const gg_walk_desc &d, const FlatView &fv, int s, long long w, int slot, int cur,
-                                             int n, int idx, int nxt, bool inc_father, unsigned long long &overflow) {
+// the walk made its choice at step s over n candidates: its outputs; true when it goes on (to level s + 1 or the tail)
+__device__ __forceinline__ bool flat_record_choice(const gg_walk_desc &d, int s, long long w, int cur, int n, int idx, int nxt,
+                                                   bool inc_father, unsigned long long &overflow) {
     if (d.max_path > 0 && d.paths && s + 1 < d.max_path) d.paths[(size_t)w * (size_t)d.max_path + s + 1] = nxt;
     d.wsteps[w] = s + 1;
     d.wsuml[w] = d.wsuml[w] + n;
@@ -541,9 +562,17 @@ __device__ __forceinline__ void flat_advance(const gg_walk_desc &d, const FlatVi
         d.samples[w] = cur; d.status[w] = GG_DONE;
         if (d.path_len) d.path_len[w] = s + 2;
         if (d.max_path > 0 && s + 2 > d.max_path) overflow += 1;
-    } else {
+        return false;
+    }
+    return true;
+}
+
+// lane 0: the walk made its choice at step s over n candidates
+__device__ __forceinline__ void flat_advance(const gg_walk_desc &d, const FlatView &fv, int s, long long w, int slot, int cur,
+                                             int n, int idx, int nxt, bool inc_father, unsigned long long &overflow) {
+    if (flat_record_choice(d, s, w, cur, n, idx, nxt, inc_father, overflow)) {
         const int4 rec = make_int4((int)w, nxt, cur, slot);
-        if (s < fv.steps) fv.list[(s + 1) & 1][atomicAdd(GG_FCTR(fv, s + 1, 0), 1u)] = rec;
+        if (s < fv.steps) level_list(fv, s + 1)[atomicAdd(GG_FCTR(fv, s + 1, 0), 1u)] = rec;
         else fv.tail[atomicAdd(fv.ctr, 1u)] = rec;
     }
 }
@@ -628,24 +657,124 @@ __global__ void __launch_bounds__(256) flat_start_kernel(const __grid_constant__
     }
 }
 
+// ---- shared levels: (1) flat_dedupe_kernel, thread per record: the record's key (root slot, node) goes into the level's
+// hash table; the record that inserts a key owns its item (candidate list + CDF); score-cached (hub) nodes go to the hub
+// list as in flat_enum_kernel and run per walk.  (2) flat_enum_kernel<true> + flat_choose_kernel<C, true>: the owners' lists
+// and their CDFs.  (3) flat_draw_kernel, thread per record: the walk's uniform inverts its item's CDF.
+__device__ __forceinline__ unsigned long long share_hash(unsigned long long key, unsigned long long mask) {
+    return ((key * 0x9E3779B97F4A7C15ull) >> 20) & mask;
+}
+
+// warp-aggregated append of `v` for the lanes with `take` (one atomic per warp)
+template <class T>
+__device__ __forceinline__ void warp_append(bool take, T *list, unsigned *cnt, const T &v, int lane) {
+    const unsigned mk = __ballot_sync(FULL, take);
+    if (!mk) return;
+    const int leader = __ffs(mk) - 1;
+    unsigned base = 0;
+    if (lane == leader) base = atomicAdd(cnt, (unsigned)__popc(mk));
+    base = __shfl_sync(FULL, base, leader);
+    if (take) list[base + __popc(mk & ((1u << lane) - 1u))] = v;
+}
+
+__global__ void __launch_bounds__(256) flat_dedupe_kernel(const __grid_constant__ gg_walk_desc d, const FlatView fv, const int s) {
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    const unsigned nA = *GG_FCTR(fv, s, 0);
+    if (blockIdx.x * blockDim.x >= nA) return;             // warp-uniform below: whole warps leave together
+    bool hub = false, owner = false;
+    if (i < nA) {
+        const int4 rec = level_list(fv, s)[i];
+        const int cur = rec.y, slot = rec.w;
+        hub = d.edge_score && (d.indptr[cur + 1] - d.indptr[cur]) >= d.hub_threshold;
+        int h = -1;
+        if (!hub) {
+            const unsigned long long key = (unsigned long long)slot * (unsigned long long)d.n_node + (unsigned long long)cur;
+            unsigned long long p = share_hash(key, fv.tbl_mask);
+            for (;;) {                                     // linear probing; the table has >= 2 slots per record
+                const unsigned long long old = atomicCAS(fv.keys + p, ~0ull, key);
+                if (old == ~0ull) { owner = true; fv.owner[p] = (int)i; break; }
+                if (old == key) break;
+                p = (p + 1) & fv.tbl_mask;
+            }
+            h = (int)p;
+        }
+        fv.rec_slot[i] = h;
+    }
+    const int item = (int)i;
+    warp_append(hub, fv.hub, GG_FCTR(fv, s, 1), item, lane);
+    warp_append(owner, fv.uniq, GG_FCTR(fv, s, 2), item, lane);
+}
+
+__global__ void __launch_bounds__(256) flat_draw_kernel(const __grid_constant__ gg_walk_desc d, const FlatView fv, const int s) {
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    const unsigned nA = *GG_FCTR(fv, s, 0);
+    if (blockIdx.x * blockDim.x >= nA) return;
+    unsigned long long overflow = 0;
+    unsigned steps = 0, suml = 0;
+    bool go_on = false;
+    int4 rec = make_int4(0, 0, 0, 0);
+    if (i < nA) {
+        const int h = fv.rec_slot[i];
+        if (h >= 0) {                                      // (hub items: done per walk by flat_choose_kernel)
+            rec = level_list(fv, s)[i];
+            const long long w = rec.x;
+            const int cur = rec.y, slot = rec.w;
+            const int item = fv.owner[h];
+            const int nrec = fv.item_n[item];
+            const int n = nrec & 0x3fffffff;
+            if (n == 0) {
+                flat_void(d, s, w);
+            } else {
+                const bool inc_father = (nrec >> 30) & 1;
+                int idx = 0;
+                if (n > 1) {
+                    uint32_t a, b;
+                    philox4x32_10((uint32_t)d.roots[slot], (uint32_t)(w - __ldg(d.walk_ptr + slot)), (uint32_t)s, d.pass_tag,
+                                  (uint32_t)d.seed, (uint32_t)(d.seed >> 32), a, b);
+                    idx = cdf_search_raw(fv.pool_cdf + (size_t)item * (size_t)(fv.stride + 1), n, u53(a, b));
+                }
+                const int nxt = fv.pool_ids[(size_t)item * (size_t)fv.stride + idx];
+                go_on = flat_record_choice(d, s, w, cur, n, idx, nxt, inc_father, overflow);
+                rec = make_int4((int)w, nxt, cur, slot);
+                steps = 1; suml = (unsigned)n;
+            }
+        }
+    }
+    if (s < fv.steps) warp_append(go_on, level_list(fv, s + 1), GG_FCTR(fv, s + 1, 0), rec, lane);
+    else warp_append(go_on, fv.tail, fv.ctr, rec, lane);
+    steps = __reduce_add_sync(FULL, steps); suml = __reduce_add_sync(FULL, suml);
+    const unsigned over = __reduce_add_sync(FULL, (unsigned)overflow);
+    if (lane == 0) {
+        if (steps) atomicAdd(d.counters + GG_CNT_RAW_STEPS, (unsigned long long)steps);
+        if (suml) atomicAdd(d.counters + GG_CNT_RAW_SUML, (unsigned long long)suml);
+        if (over) atomicAdd(d.counters + GG_CNT_PATH_OVERFLOW, (unsigned long long)over);
+    }
+}
+
 constexpr int FLAT_ENUM_WARPS = 8;
+// SHARED: the level's distinct keys only (fv.uniq, from flat_dedupe_kernel); the item keeps its list length and father flag
+// for flat_choose_kernel / flat_draw_kernel and finishes no walk itself
+template <bool SHARED>
 __global__ void __launch_bounds__(FLAT_ENUM_WARPS * 32, 6) flat_enum_kernel(const __grid_constant__ gg_walk_desc d,
                                                                             const FlatView fv, const int s) {
     const int lane = threadIdx.x & 31;
     const unsigned gw = blockIdx.x * FLAT_ENUM_WARPS + (threadIdx.x >> 5), nwarps = gridDim.x * FLAT_ENUM_WARPS;
-    const int4 *A = fv.list[s & 1];
-    const unsigned nA = *GG_FCTR(fv, s, 0);
+    const int4 *A = level_list(fv, s);
+    const unsigned nA = SHARED ? *GG_FCTR(fv, s, 2) : *GG_FCTR(fv, s, 0);
     Stage stg;
     stg.buf = nullptr; stg.bar = nullptr; stg.phase = 0u; stg.on = false;
     unsigned long long raw_steps = 0, raw_suml = 0, overflow = 0;
-    int4 rec_next = (gw < nA) ? A[gw] : make_int4(0, 0, 0, 0);
-    for (unsigned i = gw; i < nA; i += nwarps) {
+    int4 rec_next = (gw < nA) ? A[SHARED ? fv.uniq[gw] : gw] : make_int4(0, 0, 0, 0);
+    for (unsigned j = gw; j < nA; j += nwarps) {
+        const unsigned i = SHARED ? (unsigned)fv.uniq[j] : j;
         const int4 rec = rec_next;
-        if (i + nwarps < nA) rec_next = A[i + nwarps];     // the next item's record is in flight while this one is enumerated
+        if (j + nwarps < nA) rec_next = A[SHARED ? fv.uniq[j + nwarps] : j + nwarps];   // the next item's record is in flight while this one is enumerated
         const long long w = rec.x;
         const int cur = rec.y, prev = rec.z, slot = rec.w;
         const long long a0 = d.indptr[cur], a1 = d.indptr[cur + 1];
-        if (d.edge_score && (a1 - a0) >= d.hub_threshold) {          // score-cached node: the whole step runs in flat_choose_kernel
+        if (!SHARED && d.edge_score && (a1 - a0) >= d.hub_threshold) {   // score-cached node: the whole step runs in flat_choose_kernel
             if (lane == 0) { fv.hub[atomicAdd(GG_FCTR(fv, s, 1), 1u)] = (int)i; fv.item_n[i] = 0; }
             continue;
         }
@@ -657,7 +786,9 @@ __global__ void __launch_bounds__(FLAT_ENUM_WARPS * 32, 6) flat_enum_kernel(cons
         float m = 0.0f;
         enumerate_children<UNR>(d, tb, a0, a1, false, ids, nullptr, lane, n, m, stg);
         __syncwarp();
-        if (n == 0) {
+        if (SHARED) {
+            if (lane == 0) fv.item_n[i] = n | (inc_father ? (1 << 30) : 0);
+        } else if (n == 0) {
             if (lane == 0) { flat_void(d, s, w); fv.item_n[i] = 0; }
         } else if (n == 1) {
             // softmax = [1.0], cdf = [1.0] and 1.0 > u for every u in [0, 1): index 0, no score, no draw needed
@@ -675,7 +806,9 @@ __global__ void __launch_bounds__(FLAT_ENUM_WARPS * 32, 6) flat_enum_kernel(cons
     }
 }
 
-template <int CPL>
+// SHARED: the items that are not score-cached are the level's distinct keys (fv.uniq); their CDF is stored for
+// flat_draw_kernel instead of being drawn from.  Hub items are the same either way.
+template <int CPL, bool SHARED>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose_kernel(const __grid_constant__ gg_walk_desc d,
                                                                                         const FlatView fv, const int s) {
     extern __shared__ __align__(16) unsigned char walk_smem[];
@@ -697,8 +830,8 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose
     const long long gw = (long long)blockIdx.x * WARPS_PER_CTA + wid;
     int *g_ids = reinterpret_cast<int *>(d.scratch) + (size_t)gw * 2 * (size_t)d.max_cand;
     float *g_sc = reinterpret_cast<float *>(g_ids + d.max_cand);
-    const int4 *A = fv.list[s & 1];
-    const unsigned nA = *GG_FCTR(fv, s, 0), nH = *GG_FCTR(fv, s, 1);
+    const int4 *A = level_list(fv, s);
+    const unsigned nA = SHARED ? *GG_FCTR(fv, s, 2) : *GG_FCTR(fv, s, 0), nH = *GG_FCTR(fv, s, 1);
     const uint32_t k0 = (uint32_t)d.seed, k1 = (uint32_t)(d.seed >> 32);
     unsigned long long raw_steps = 0, raw_suml = 0, overflow = 0, rows_gathered = 0;
     unsigned int cyc[7] = {0, 0, 0, 0, 0, 0, 0};
@@ -713,14 +846,19 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_pulls) break;
         const bool hub_item = j < nH;
-        unsigned i = hub_item ? (unsigned)fv.hub[j] : (j - nH) * FLAT_CHUNK;
-        const unsigned i_end = hub_item ? i + 1 : ((i + FLAT_CHUNK < nA) ? i + FLAT_CHUNK : nA);
-        int4 rec_next = A[i];
-        int n_next = hub_item ? 0 : fv.item_n[i];
-        for (; i < i_end; ++i) {
+        unsigned p = hub_item ? 0u : (j - nH) * FLAT_CHUNK;
+        const unsigned p_end = hub_item ? 1u : ((p + FLAT_CHUNK < nA) ? p + FLAT_CHUNK : nA);
+        unsigned i_next = hub_item ? (unsigned)fv.hub[j] : (SHARED ? (unsigned)fv.uniq[p] : p);
+        int4 rec_next = A[i_next];
+        int n_next = hub_item ? 0 : fv.item_n[i_next];
+        for (; p < p_end; ++p) {
+            const unsigned i = i_next;
             const int4 rec = rec_next;
             const int nrec = n_next;
-            if (i + 1 < i_end) { rec_next = A[i + 1]; n_next = fv.item_n[i + 1]; }
+            if (p + 1 < p_end) {
+                i_next = SHARED ? (unsigned)fv.uniq[p + 1] : p + 1;
+                rec_next = A[i_next]; n_next = fv.item_n[i_next];
+            }
             if (!hub_item && (nrec & 0x3fffffff) < 2) continue;      // finished by flat_enum_kernel, or a hub item
             const long long w = rec.x;
             const int cur = rec.y, prev = rec.z, slot = rec.w;
@@ -751,6 +889,11 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose
                 score_list<CPL>(d.emb, d.bias, d.ld, c4, ids, s_sc, n, cur, lane);
                 rows_gathered += 1u + (unsigned)n;
                 const float m = list_max(s_sc, n, lane);
+                if (SHARED) {
+                    cdf_store_raw<UNR>(s_sc, n, m, fv.pool_cdf + (size_t)i * (size_t)(fv.stride + 1), lane);
+                    __syncwarp();
+                    continue;
+                }
                 philox4x32_10((uint32_t)root, k, (uint32_t)s, d.pass_tag, k0, k1, a, b);
                 idx = choose_index(s_sc, n, m, u53(a, b), lane);
                 nxt = ids[idx];
@@ -784,9 +927,25 @@ size_t flat_layout(void *buf, long long n_walks, int hub_threshold, int steps, F
     int4 *l0 = (int4 *)take(16 * W), *l1 = (int4 *)take(16 * W), *tail = (int4 *)take(16 * W);
     int *hub = (int *)take(4 * W), *item_n = (int *)take(4 * W);
     int *pool = (int *)take(4 * W * (size_t)stride);
+    // shared levels: a table of >= 2 slots per record (W = 322 k: 2^20 slots, 12 MB), the owners' CDF slab (332 MB)
+    unsigned long long cap = 0;
+    unsigned long long *keys = nullptr;
+    int *owner = nullptr, *rec_slot = nullptr, *uniq = nullptr;
+    double *cdf = nullptr;
+    if (any_level_shared(steps)) {
+        cap = 1;
+        while (cap < 2 * (unsigned long long)W) cap <<= 1;
+        keys = (unsigned long long *)take(8 * cap);
+        owner = (int *)take(4 * cap);
+        rec_slot = (int *)take(4 * W);
+        uniq = (int *)take(4 * W);
+        cdf = (double *)take(8 * W * (size_t)(stride + 1));
+    }
     if (fv) {
         fv->ctr = ctr; fv->list[0] = l0; fv->list[1] = l1; fv->tail = tail; fv->hub = hub;
         fv->item_n = item_n; fv->pool_ids = pool; fv->stride = stride; fv->steps = steps;
+        fv->keys = keys; fv->owner = owner; fv->rec_slot = rec_slot; fv->uniq = uniq; fv->pool_cdf = cdf;
+        fv->tbl_mask = cap ? cap - 1 : 0;
     }
     return off;
 }
@@ -1041,14 +1200,30 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
             gg::flat_start_kernel<<<(unsigned)((d.n_walks + 255) / 256), 256, 0, st>>>(d, fv);
             GG_CHECK(cudaGetLastError());
             const int enum_ctas = gg::sm_count() * 8;
+            const unsigned rec_ctas = (unsigned)((d.n_walks + 255) / 256);
+            GG_REQUIRE(!gg::any_level_shared(d.flat_steps) || d.n_node > 0, "n_node missing");
             for (int s = 1; s <= d.flat_steps; ++s) {
-                gg::flat_enum_kernel<<<enum_ctas, gg::FLAT_ENUM_WARPS * 32, 0, st>>>(d, fv, s);
+                const bool shared = gg::level_shared(s);
+                if (shared) {
+                    GG_CHECK(cudaMemsetAsync(fv.keys, 0xff, sizeof(unsigned long long) * (size_t)(fv.tbl_mask + 1), st));
+                    gg::flat_dedupe_kernel<<<rec_ctas, 256, 0, st>>>(d, fv, s);
+                    GG_CHECK(cudaGetLastError());
+                    gg::flat_enum_kernel<true><<<enum_ctas, gg::FLAT_ENUM_WARPS * 32, 0, st>>>(d, fv, s);
+                } else {
+                    gg::flat_enum_kernel<false><<<enum_ctas, gg::FLAT_ENUM_WARPS * 32, 0, st>>>(d, fv, s);
+                }
                 GG_CHECK(cudaGetLastError());
                 switch (cpl) {
 #define GG_FLAT(C)                                                                                                    \
-    GG_CHECK(cudaFuncSetAttribute(gg::flat_choose_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,            \
-                                  gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP));                                      \
-    gg::flat_choose_kernel<C><<<ctas, gg::WARPS_PER_CTA * 32, gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP, st>>>(d, fv, s)
+    if (shared) {                                                                                                    \
+        GG_CHECK(cudaFuncSetAttribute(gg::flat_choose_kernel<C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
+                                      gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP));                                  \
+        gg::flat_choose_kernel<C, true><<<ctas, gg::WARPS_PER_CTA * 32, gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP, st>>>(d, fv, s); \
+    } else {                                                                                                         \
+        GG_CHECK(cudaFuncSetAttribute(gg::flat_choose_kernel<C, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+                                      gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP));                                  \
+        gg::flat_choose_kernel<C, false><<<ctas, gg::WARPS_PER_CTA * 32, gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP, st>>>(d, fv, s); \
+    }
                     case 1: GG_FLAT(1); break;
                     case 2: GG_FLAT(2); break;
                     case 4: GG_FLAT(4); break;
@@ -1057,6 +1232,10 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
                     default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256)", d.ld); return 2;
                 }
                 GG_CHECK(cudaGetLastError());
+                if (shared) {
+                    gg::flat_draw_kernel<<<rec_ctas, 256, 0, st>>>(d, fv, s);
+                    GG_CHECK(cudaGetLastError());
+                }
             }
             tail_mode = 1;
         }

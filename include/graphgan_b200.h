@@ -129,7 +129,9 @@ typedef struct gg_walk_desc {
                                  * 0..W-1, e.g. expensive roots first); results do not depend on it (Philox mode) */
     /* optional level-synchronous steps (needs the depth-1 reuse): all unfinished walks take step s together -- one
        kernel enumerates the candidate lists, one gathers the candidates' rows and draws -- for steps 1..flat_steps;
-       the persistent kernel finishes the walks that are still alive after that.  Identical results. */
+       the persistent kernel finishes the walks that are still alive after that.  On the levels the library shares
+       (step 2 by default) the walks of a root that stand on the same node draw from one candidate list and CDF,
+       keyed by (root slot, node): n_node must be set.  Identical results. */
     void *flat_buf;             /* device scratch of gg_walk_flat_bytes(n_walks, hub_threshold, flat_steps) bytes */
     int64_t flat_bytes;
     int32_t flat_steps;         /* 0 = off (persistent kernel only); <= 14 */

@@ -18,6 +18,8 @@ VARIANTS = {
     "occ4": ["GG_WALK_MIN_CTAS=4", "GG_SC_CAP=1024", "GG_UNR=2"],    # 4 CTAs/SM at 64 registers
     "occ5": ["GG_WALK_MIN_CTAS=5"],
     "unr2": ["GG_UNR=2"],
+    "share0": ["GG_SHARE_LEVELS=0"],              # no shared level: every level runs flat_enum + flat_choose per walk
+    "share23": ["GG_SHARE_LEVELS=0xC"],           # levels 2 and 3 shared (default: level 2)
 }
 
 
