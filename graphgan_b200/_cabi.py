@@ -9,7 +9,7 @@ import os
 from . import _build
 
 _LIB = None
-ABI_VERSION = 4      # == GG_ABI_VERSION of include/graphgan_b200.h
+ABI_VERSION = 5      # == GG_ABI_VERSION of include/graphgan_b200.h
 
 
 class GGError(RuntimeError):
@@ -63,6 +63,8 @@ SIGNATURES = {
     "gg_pair_grad_ex": (C.c_int, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _I32, _F, _P, _P, _P, _P, _P, _P, _I64, _I32, _P]),
     "gg_grad_buf_floats": (_I64, [_I32, _I32]),
     "gg_grad_merge": (C.c_int, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P]),
+    "gg_grad_merge_scratch_bytes": (C.c_int, [_I32, _I32, _I32, C.POINTER(_I64)]),
+    "gg_grad_merge_ex": (C.c_int, [_I32, _I32, _I32, _P, _P, _P, _P, _P, _P, _P, _I64, _I32, _P]),
     "gg_comm_unique_id": (C.c_int, [_P]),
     "gg_comm_init": (C.c_int, [_P, _I32, _I32, C.POINTER(C.c_void_p)]),
     "gg_comm_destroy": (C.c_int, [_P]),
@@ -74,6 +76,12 @@ SIGNATURES = {
                             _F, _F, _F, _F, _P]),
     "gg_dp_train_steps": (C.c_int, [_P, _I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _I32,
                                    _P, _P, _P, _P, _P, _F, _F, _F, _F, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
+    "gg_dp_scratch_bytes": (C.c_int, [_I32, _I32, _I32, C.POINTER(_I64)]),
+    "gg_dp_step_ex": (C.c_int, [_P, _I32, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _I32, _P, _P, _P, _P, _P,
+                               _F, _F, _F, _F, _P, _I64, _I32, _P]),
+    "gg_dp_train_steps_ex": (C.c_int, [_P, _I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _I32,
+                                      _P, _P, _P, _P, _P, _F, _F, _F, _F, C.POINTER(C.c_float), C.POINTER(C.c_float), _P, _I64,
+                                      _I32, _P]),
     "gg_set_adam_path": (C.c_int, [C.c_char_p]),
     "gg_adam_apply": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _F, _F, _F, _F, _P]),
     "gg_train_steps": (C.c_int, [_I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P,

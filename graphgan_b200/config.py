@@ -17,7 +17,7 @@ n_epochs_gen = 30                   # generator inner loops per outer loop
 dis_interval = n_epochs_dis         # resample discriminator data every this many inner loops
 gen_interval = n_epochs_gen         # same for the generator
 batch_size_dis = 64                 # pairs per discriminator step (any size; above 1024 the gradient runs multi-CTA)
-batch_size_gen = 64                 # pairs per generator step (likewise; one GPU only above 1024)
+batch_size_gen = 64                 # pairs per generator step (likewise, also data parallel under torchrun)
 lr_dis = 1e-3                       # Adam learning rates
 lr_gen = 1e-3
 lambda_dis = 1e-5                   # l2 weights of the two losses

@@ -8,6 +8,9 @@
 //                (rows[cap, ld] | bias[cap] | ids[cap] | n_unique: a few KB -- latency bound, which NVSwitch is good at)
 //                ->  deterministic rank-major merge (gg_grad_merge)  ->  the same K3 sweep on every rank.
 //
+// Above GG_MAX_BATCH pairs (gg_dp_step_ex / gg_dp_train_steps_ex, NCCL only) the slice gradient and the merge are the
+// multi-CTA gg_pair_grad_ex and gg_grad_merge_ex (grad_multi.cu), with the same entry order and sums.
+//
 // An all-gather + ordered merge instead of a float all-reduce: (i) the dense [N, ld] gradient is 512 MB per step at
 // C3 against 64 KB compact, and (ii) every replica adds the same floats in the same order, so replicas stay
 // BIT-IDENTICAL without ever broadcasting parameters.  All four stages are enqueued on the caller's stream from C
@@ -336,6 +339,122 @@ extern "C" int gg_dp_train_steps(void *comm, int32_t mode, int64_t n_rows, const
         int rc = gg_dp_step(comm, mode, (int32_t)(end - start), node_id + start, node_neighbor_id + start, aux + start, n_node, ld,
                             emb, m_emb, v_emb, bias, m_bias, v_bias, lambda, local_buf, gathered_buf, cap, n_unique, uniq_ids,
                             grad_rows, grad_bias, row_slot, lr_t, beta1, beta2, eps, stream);
+        if (rc) return rc;
+        volatile float p1 = *beta1_power * beta1, p2 = *beta2_power * beta2;
+        *beta1_power = p1;
+        *beta2_power = p2;
+    }
+    return 0;
+}
+
+// ---------------------------------------------------------------- the same step for any batch size
+// Slice gradient (gg_pair_grad_ex: one CTA up to GG_MAX_BATCH pairs, multi-CTA above), the same single ncclAllGather, the
+// multi-CTA merge (gg_grad_merge_ex) and the Adam sweep.  The two scratch users run one after the other on the stream and
+// share one buffer.
+static const int64_t DP_MAX_PAIRS = (1ll << 30) - 4096;   // == the multi-CTA gradient's limit
+
+extern "C" int gg_dp_scratch_bytes(int32_t world, int32_t n_pairs, int32_t ld, int64_t *bytes) {
+    GG_REQUIRE(bytes, "null pointer");
+    GG_REQUIRE(world >= 1, "world must be >= 1");
+    GG_REQUIRE(n_pairs > 0 && n_pairs <= DP_MAX_PAIRS, "n_pairs must be in 1 .. 2^30 - 4096");
+    const int64_t slice = (n_pairs + (int64_t)world - 1) / world;
+    int64_t grad = 0, merge = 0;
+    int rc = gg_pair_grad_scratch_bytes((int32_t)slice, ld, &grad);
+    if (rc) return rc;
+    rc = gg_grad_merge_scratch_bytes(world, (int32_t)(2 * slice), ld, &merge);
+    if (rc) return rc;
+    *bytes = grad > merge ? grad : merge;
+    return 0;
+}
+
+extern "C" int gg_dp_step_ex(void *comm, int32_t mode, int32_t n_pairs, const int32_t *node_id, const int32_t *node_neighbor_id,
+                             const float *aux, int64_t n_node, int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias,
+                             float *m_bias, float *v_bias, float lambda, float *local_buf, float *gathered_buf, int32_t cap,
+                             int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot,
+                             float lr_t, float beta1, float beta2, float eps, void *scratch, int64_t scratch_bytes, int32_t flags,
+                             void *stream) {
+    GG_REQUIRE(comm, "null communicator");
+    GG_REQUIRE((flags & ~GG_GRAD_MULTI_CTA) == 0, "unknown flags");
+    if (n_pairs > 0 && n_pairs <= GG_MAX_BATCH && !flags)
+        return gg_dp_step(comm, mode, n_pairs, node_id, node_neighbor_id, aux, n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias,
+                          lambda, local_buf, gathered_buf, cap, n_unique, uniq_ids, grad_rows, grad_bias, row_slot, lr_t, beta1,
+                          beta2, eps, stream);
+    gg::Comm *c = (gg::Comm *)comm;
+    GG_REQUIRE(!c->p2p, "the peer-memory transport takes at most GG_MAX_BATCH pairs per step (use the NCCL transport: "
+                        "gg_comm_use_p2p(comm, 0))");
+    GG_REQUIRE(n_pairs > 0 && n_pairs <= DP_MAX_PAIRS, "n_pairs must be in 1 .. 2^30 - 4096");
+    GG_REQUIRE(mode == 0 || mode == 1, "mode must be 0 (discriminator) or 1 (generator)");
+    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(node_id && node_neighbor_id && aux && local_buf && gathered_buf, "null pointer");
+    GG_REQUIRE(cap >= 2 * (((int64_t)n_pairs + c->world - 1) / c->world), "cap too small: need 2 * ceil(n_pairs / world)");
+    int lo, hi;
+    block_range(n_pairs, c->rank, c->world, &lo, &hi);
+    // every size check before the collective, so that a bad call fails on every rank without communicating
+    int64_t need_grad = 0, need_merge = 0;
+    const bool multi_grad = hi - lo > GG_MAX_BATCH || (flags & GG_GRAD_MULTI_CTA);
+    if (hi > lo && multi_grad) {
+        int rc = gg_pair_grad_scratch_bytes(hi - lo, ld, &need_grad);
+        if (rc) return rc;
+    }
+    int rc = gg_grad_merge_scratch_bytes(c->world, cap, ld, &need_merge);
+    if (rc) return rc;
+    GG_REQUIRE(scratch && scratch_bytes >= need_grad && scratch_bytes >= need_merge,
+               "scratch is null or smaller than gg_dp_scratch_bytes");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t nf = gg_grad_buf_floats(cap, ld);
+    float *rows_p = local_buf, *bias_p = local_buf + (size_t)cap * ld;
+    int32_t *ids_p = (int32_t *)(bias_p + cap), *nu_p = ids_p + cap;
+    if (hi > lo) {      // this rank's slice, written straight into its block; the generator loss is a mean over n_pairs
+        rc = gg_pair_grad_ex(mode, hi - lo, n_pairs, node_id + lo, node_neighbor_id + lo, aux + lo, emb, bias, ld, lambda, nu_p,
+                             ids_p, rows_p, bias_p, row_slot, scratch, scratch_bytes, flags, stream);
+        if (rc) return rc;
+    } else {
+        GG_CHECK(cudaMemsetAsync(nu_p, 0, sizeof(float) * (size_t)(nf - ((size_t)cap * ld + 2 * (size_t)cap)), st));
+    }
+    GG_NCCL(gg::nccl().AllGather(local_buf, gathered_buf, (size_t)nf, gg::NCCL_FLOAT32, c->comm, st));   // the step's only collective
+    c->collectives += 1;
+    rc = gg_grad_merge_ex(c->world, cap, ld, gathered_buf, n_unique, uniq_ids, grad_rows, grad_bias, row_slot, scratch, scratch_bytes,
+                          GG_GRAD_MULTI_CTA, stream);
+    if (rc) return rc;
+    return gg_adam_apply(n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, n_unique, uniq_ids, grad_rows, grad_bias, row_slot,
+                         lr_t, beta1, beta2, eps, stream);
+}
+
+extern "C" int gg_dp_train_steps_ex(void *comm, int32_t mode, int64_t n_rows, const int64_t *start_list, int64_t n_starts,
+                                    int32_t batch_size, const int32_t *node_id, const int32_t *node_neighbor_id, const float *aux,
+                                    int64_t n_node, int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias, float *m_bias,
+                                    float *v_bias, float lambda, float *local_buf, float *gathered_buf, int32_t cap,
+                                    int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot,
+                                    float lr, float beta1, float beta2, float eps, float *beta1_power, float *beta2_power,
+                                    void *scratch, int64_t scratch_bytes, int32_t flags, void *stream) {
+    GG_REQUIRE(comm, "null communicator");
+    GG_REQUIRE(start_list && beta1_power && beta2_power, "null host pointer");
+    GG_REQUIRE((flags & ~GG_GRAD_MULTI_CTA) == 0, "unknown flags");
+    GG_REQUIRE(batch_size > 0 && batch_size <= DP_MAX_PAIRS, "batch size out of range");
+    if (batch_size <= GG_MAX_BATCH && !flags)
+        return gg_dp_train_steps(comm, mode, n_rows, start_list, n_starts, batch_size, node_id, node_neighbor_id, aux, n_node, ld, emb,
+                                 m_emb, v_emb, bias, m_bias, v_bias, lambda, local_buf, gathered_buf, cap, n_unique, uniq_ids,
+                                 grad_rows, grad_bias, row_slot, lr, beta1, beta2, eps, beta1_power, beta2_power, stream);
+    gg::Comm *c = (gg::Comm *)comm;
+    GG_REQUIRE(!c->p2p, "the peer-memory transport takes at most GG_MAX_BATCH pairs per step (use the NCCL transport: "
+                        "gg_comm_use_p2p(comm, 0))");
+    GG_REQUIRE(cap >= 2 * (((int64_t)batch_size + c->world - 1) / c->world), "cap too small: need 2 * ceil(batch_size / world)");
+    for (int64_t s = 0; s < n_starts; ++s) {
+        const int64_t start = start_list[s];
+        GG_REQUIRE(start >= 0 && start < n_rows, "start out of range");
+        const int64_t end = start + batch_size < n_rows ? start + batch_size : n_rows;
+        const int32_t n = (int32_t)(end - start);
+        // each step lays its blocks out for its own size (a short last batch of <= GG_MAX_BATCH pairs then fits the one-CTA
+        // merge); the merged result does not depend on cap
+        const int32_t step_cap = (int32_t)(2 * (((int64_t)n + c->world - 1) / c->world));
+        volatile float one_m_b2 = 1.0f - *beta2_power;       // lr_t as in gg_dp_train_steps
+        volatile float root = sqrtf(one_m_b2);
+        volatile float num = lr * root;
+        volatile float den = 1.0f - *beta1_power;
+        const float lr_t = num / den;
+        int rc = gg_dp_step_ex(comm, mode, n, node_id + start, node_neighbor_id + start, aux + start, n_node, ld, emb, m_emb, v_emb,
+                               bias, m_bias, v_bias, lambda, local_buf, gathered_buf, step_cap, n_unique, uniq_ids, grad_rows,
+                               grad_bias, row_slot, lr_t, beta1, beta2, eps, scratch, scratch_bytes, flags, stream);
         if (rc) return rc;
         volatile float p1 = *beta1_power * beta1, p2 = *beta2_power * beta2;
         *beta1_power = p1;

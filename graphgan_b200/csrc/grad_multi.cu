@@ -18,6 +18,10 @@
 //                 thread per column, the slot's contiguous terms streamed through a cp.async ring in shared memory so
 //                 that ~200 KB of loads are in flight while the adds run in entry order
 // A slot's chain is serial by contract, so the longest slot bounds the last stage (DESIGN.md section 5, K2).
+//
+// gg_grad_merge_ex (data-parallel merge of `world` compact gradients, any size) reuses stages 2 and 3 on the entries of
+// the gathered blocks (number_and_group over MergeEntries): the ids are read and their row_slot cleared in one launch,
+// first entries found by atomicMin in the next, and the sums read the rows in place through the sorted entry index.
 #include "update_dev.cuh"
 
 namespace gg {
@@ -115,20 +119,34 @@ __device__ __forceinline__ int block_excl_scan(int x) {   // MC_THREADS threads
     return excl;
 }
 
-__global__ void __launch_bounds__(MC_THREADS) mc_count_kernel(int B, const int *__restrict__ ni, const int *__restrict__ nj,
-                                                              const int *row_slot, long long *__restrict__ tile_cnt) {
+// Where the grouping stages (2, 3) read entry t's row id: the pair entries of a mini-batch, or the slots of the
+// gathered blocks of gg_grad_merge_ex (id -1: rank r has no slot s).  An absent entry is never a first occurrence and
+// sorts after every slot (key E).
+struct PairEntries {
+    int B;
+    const int *ni, *nj;
+    __device__ __forceinline__ int id(int t) const { return entry_id(t, B, ni, nj); }
+};
+struct MergeEntries {
+    const int *ids;
+    __device__ __forceinline__ int id(int t) const { return ids[t]; }
+};
+
+template <class Src>
+__global__ void __launch_bounds__(MC_THREADS) mc_count_kernel(int E, Src src, const int *row_slot, long long *__restrict__ tile_cnt) {
     const int t = blockIdx.x * MC_THREADS + threadIdx.x;
-    const int first = (t < 2 * B && row_slot[entry_id(t, B, ni, nj)] == t) ? 1 : 0;
+    const int id = t < E ? src.id(t) : -1;
+    const int first = (id >= 0 && row_slot[id] == t) ? 1 : 0;
     const int n = __syncthreads_count(first);
     if (threadIdx.x == 0) tile_cnt[blockIdx.x] = n;
 }
 
-__global__ void __launch_bounds__(MC_THREADS) mc_number_kernel(int B, const int *__restrict__ ni, const int *__restrict__ nj,
-                                                               const long long *__restrict__ tile_off, int n_tiles, int *row_slot,
-                                                               int *__restrict__ uniq_ids, int *__restrict__ n_unique) {
+template <class Src>
+__global__ void __launch_bounds__(MC_THREADS) mc_number_kernel(int E, Src src, const long long *__restrict__ tile_off, int n_tiles,
+                                                               int *row_slot, int *__restrict__ uniq_ids, int *__restrict__ n_unique) {
     const int t = blockIdx.x * MC_THREADS + threadIdx.x;
-    const int id = t < 2 * B ? entry_id(t, B, ni, nj) : 0;
-    const int first = (t < 2 * B && row_slot[id] == t) ? 1 : 0;
+    const int id = t < E ? src.id(t) : -1;
+    const int first = (id >= 0 && row_slot[id] == t) ? 1 : 0;
     const int excl = block_excl_scan(first);
     if (first) {
         const int slot = (int)tile_off[blockIdx.x] + excl;
@@ -139,11 +157,15 @@ __global__ void __launch_bounds__(MC_THREADS) mc_number_kernel(int B, const int 
 }
 
 // ---- 3: stable LSD radix sort of (slot, entry) by slot
-__global__ void __launch_bounds__(MC_THREADS) mc_keys_kernel(int B, const int *__restrict__ ni, const int *__restrict__ nj,
-                                                             const int *__restrict__ row_slot, int *__restrict__ key,
+template <class Src>
+__global__ void __launch_bounds__(MC_THREADS) mc_keys_kernel(int E, Src src, const int *__restrict__ row_slot, int *__restrict__ key,
                                                              int *__restrict__ val) {
     const long long t = (long long)blockIdx.x * MC_THREADS + threadIdx.x;
-    if (t < 2ll * B) { key[t] = row_slot[entry_id((int)t, B, ni, nj)]; val[t] = (int)t; }
+    if (t < E) {
+        const int id = src.id((int)t);
+        key[t] = id >= 0 ? row_slot[id] : E;
+        val[t] = (int)t;
+    }
 }
 
 __global__ void __launch_bounds__(MC_THREADS) mc_hist_kernel(int E, const int *__restrict__ key, int shift, int r_tiles,
@@ -339,6 +361,151 @@ __global__ void __launch_bounds__(LONG_THREADS, 1) mc_long_sums_kernel(int ld, c
     }
 }
 
+// Stages 2 + 3 on the caller's stream for E entries whose ids `src` gives, with row_slot[id] = first entry of the row:
+// slots, uniq_ids, n_unique, then the entries (val) sorted by slot (key; absent entries, key E, last).  keys <= max_key.
+// *cur: the ping-pong half that holds the sorted arrays.
+template <class Src>
+int number_and_group(const Src &src, int E, int max_key, int *row_slot, int *uniq_ids, int *n_unique, long long *tile_cnt,
+                     long long *hist, int *const key[2], int *const val[2], cudaStream_t st, int *cur) {
+    const int n_tiles = (E + MC_THREADS - 1) / MC_THREADS, r_tiles = (E + RADIX_TILE - 1) / RADIX_TILE;
+    mc_count_kernel<<<n_tiles, MC_THREADS, 0, st>>>(E, src, row_slot, tile_cnt);
+    GG_CHECK(cudaGetLastError());
+    int rc = launch_exclusive_scan_i64(tile_cnt, n_tiles, nullptr, st);
+    if (rc) return rc;
+    mc_number_kernel<<<n_tiles, MC_THREADS, 0, st>>>(E, src, tile_cnt, n_tiles, row_slot, uniq_ids, n_unique);
+    GG_CHECK(cudaGetLastError());
+    mc_keys_kernel<<<n_tiles, MC_THREADS, 0, st>>>(E, src, row_slot, key[0], val[0]);
+    GG_CHECK(cudaGetLastError());
+    int bits = 1;
+    while (bits < 31 && (max_key >> bits) != 0) ++bits;
+    int c = 0;
+    for (int shift = 0; shift < bits; shift += 8, c ^= 1) {
+        mc_hist_kernel<<<r_tiles, MC_THREADS, 0, st>>>(E, key[c], shift, r_tiles, hist);
+        GG_CHECK(cudaGetLastError());
+        rc = launch_exclusive_scan_i64(hist, 256ll * r_tiles, nullptr, st);
+        if (rc) return rc;
+        mc_scatter_kernel<<<r_tiles, MC_THREADS, 0, st>>>(E, key[c], val[c], shift, r_tiles, hist, key[c ^ 1], val[c ^ 1]);
+        GG_CHECK(cudaGetLastError());
+    }
+    *cur = c;
+    return 0;
+}
+
+// ---------------------------------------------------------------- multi-CTA data-parallel merge (gg_grad_merge_ex)
+// The contract of grad_merge_body (update_dev.cuh) for any number of entries: entry t = r * cap + s for s < nu_r, slots
+// in first-occurrence order over t, per slot one +0-started __fadd_rn chain over its entries in increasing t (= rank
+// order).  A rank's block holds every id once, so a slot has at most `world` entries: one 8-lane group per slot sums
+// it, reading the rows in the gathered buffer through the sorted entry index (no term copy, no long-slot path).
+struct MergeScratch {
+    int *ids;                  // [E] entry -> row id, -1 where s >= nu_r
+    long long *tile_cnt;       // [n_tiles + 1]
+    int *key[2], *val[2];      // [E] radix ping-pong: slot (E = absent) and entry index
+    long long *hist;           // [256 * radix tiles + 1]
+    int *off;                  // [E + 1] slot -> first grouped position
+    size_t bytes;
+};
+
+MergeScratch carve_merge(char *base, long long E) {
+    const long long n_tiles = (E + MC_THREADS - 1) / MC_THREADS, r_tiles = (E + RADIX_TILE - 1) / RADIX_TILE;
+    MergeScratch s;
+    size_t at = 0;
+    auto take = [&](size_t bytes) { char *p = base ? base + at : nullptr; at += align_up(bytes); return p; };
+    s.ids = (int *)take(4 * E);
+    s.tile_cnt = (long long *)take(8 * (n_tiles + 1));
+    for (int k = 0; k < 2; ++k) { s.key[k] = (int *)take(4 * E); s.val[k] = (int *)take(4 * E); }
+    s.hist = (long long *)take(8 * (256 * r_tiles + 1));
+    s.off = (int *)take(4 * (E + 1));
+    s.bytes = at;
+    return s;
+}
+
+__host__ __device__ inline size_t merge_stride(int cap, int ld) { return (size_t)cap * ld + 2 * (size_t)cap + 4; }   // == gg_grad_buf_floats
+
+// ---- merge 1: every entry's id, and row_slot[id] = -1 for every id present (it may still hold this rank's local slots
+// from the slice gradient).  A launch of its own: the first-occurrence atomicMin below must see all of them cleared.
+__global__ void __launch_bounds__(256) mg_ids_kernel(int E, int cap, int ld, const float *__restrict__ gathered, int *__restrict__ ids,
+                                                     int *row_slot) {
+    const size_t stride = merge_stride(cap, ld);
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < E; t += (long long)gridDim.x * blockDim.x) {
+        const int r = (int)(t / cap), s = (int)(t - (long long)r * cap);
+        const float *tail = gathered + (size_t)r * stride + (size_t)cap * ld;       // bias | ids | n_unique
+        const int nu = __float_as_int(__ldg(tail + 2 * (size_t)cap));
+        const int id = s < nu ? __float_as_int(__ldg(tail + cap + s)) : -1;
+        ids[t] = id;
+        if (id >= 0) row_slot[id] = -1;
+    }
+}
+
+// ---- merge 2: first entry of every row (row_slot = -1 = UINT_MAX everywhere it is read)
+__global__ void __launch_bounds__(256) mg_first_kernel(int E, const int *__restrict__ ids, int *row_slot) {
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < E; t += (long long)gridDim.x * blockDim.x) {
+        const int id = ids[t];
+        if (id >= 0) atomicMin(reinterpret_cast<unsigned *>(row_slot) + id, (unsigned)t);
+    }
+}
+
+// ---- merge 3: slot -> [off[u], off[u + 1]) in grouped order (both ends written; neighbours write equal values)
+__global__ void __launch_bounds__(256) mg_offsets_kernel(int E, const int *__restrict__ key, int *__restrict__ off) {
+    for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < E; p += (long long)gridDim.x * blockDim.x) {
+        const int u = key[p];
+        if (u == E) continue;
+        if (p == 0 || key[p - 1] != u) off[u] = (int)p;
+        if (p == E - 1 || key[p + 1] != u) off[u + 1] = (int)p + 1;
+    }
+}
+
+// ---- merge 4: sums, one 8-lane group per slot (columns in passes of 64, four entries' rows in flight), entries in t order
+__global__ void __launch_bounds__(256) mg_sums_kernel(int cap, int ld, const float *__restrict__ gathered, const int *__restrict__ n_unique,
+                                                      const int *__restrict__ off, const int *__restrict__ val,
+                                                      float *__restrict__ grad_rows, float *__restrict__ grad_bias) {
+    const int g = threadIdx.x & 7;
+    const long long gid = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 3;
+    const long long ngrp = ((long long)gridDim.x * blockDim.x) >> 3;
+    const int U = *n_unique;
+    const size_t stride = merge_stride(cap, ld);
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+    auto row_of = [&](int t) {        // rows[s] of rank r's block
+        const int r = t / cap;
+        return gathered + (size_t)r * stride + (size_t)(t - r * cap) * ld;
+    };
+    for (long long u = gid; u < U; u += ngrp) {
+        const int lo = off[u], n = off[u + 1] - lo;
+        for (int c0 = 0; c0 < ld; c0 += 64) {
+            const int c = c0 + 4 * g;
+            const bool two = c + 32 < ld;
+            float4 acc0 = z, acc1 = z;
+            for (int r = 0; r < n; r += 4) {
+                float4 o0[4], o1[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const bool in = r + e < n;
+                    const float *tp = row_of(in ? val[lo + r + e] : 0) + c;
+                    o0[e] = in ? ldg4(tp) : z;
+                    o1[e] = (in && two) ? ldg4(tp + 32) : z;
+                }
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    if (r + e >= n) break;
+                    acc0.x = __fadd_rn(acc0.x, o0[e].x); acc0.y = __fadd_rn(acc0.y, o0[e].y);
+                    acc0.z = __fadd_rn(acc0.z, o0[e].z); acc0.w = __fadd_rn(acc0.w, o0[e].w);
+                    acc1.x = __fadd_rn(acc1.x, o1[e].x); acc1.y = __fadd_rn(acc1.y, o1[e].y);
+                    acc1.z = __fadd_rn(acc1.z, o1[e].z); acc1.w = __fadd_rn(acc1.w, o1[e].w);
+                }
+            }
+            *reinterpret_cast<float4 *>(grad_rows + (size_t)u * ld + c) = acc0;
+            if (two) *reinterpret_cast<float4 *>(grad_rows + (size_t)u * ld + c + 32) = acc1;
+        }
+        if (g == 0) {
+            float gb = 0.0f;
+            for (int r = 0; r < n; ++r) {
+                const int t = val[lo + r], k = t / cap;
+                gb = __fadd_rn(gb, __ldg(gathered + (size_t)k * stride + (size_t)cap * ld + (t - k * cap)));
+            }
+            grad_bias[u] = gb;
+        }
+    }
+}
+
 }  // namespace
 }  // namespace gg
 
@@ -369,32 +536,14 @@ extern "C" int gg_pair_grad_ex(int32_t mode, int32_t n_pairs, int32_t batch_tota
     const gg::Scratch s = gg::carve((char *)scratch, n_pairs, ld);
     cudaStream_t st = (cudaStream_t)stream;
     const int B = n_pairs, E = 2 * n_pairs;
-    const int n_tiles = (E + gg::MC_THREADS - 1) / gg::MC_THREADS, r_tiles = (E + gg::RADIX_TILE - 1) / gg::RADIX_TILE;
     const int grid = gg::sm_count() * 8;
     gg::mc_forward_kernel<<<grid, 256, 0, st>>>(mode, B, batch_total > 0 ? batch_total : B, node_id, node_neighbor_id, aux, emb,
                                                  bias, ld, s.delta, row_slot);
     GG_CHECK(cudaGetLastError());
-    gg::mc_count_kernel<<<n_tiles, gg::MC_THREADS, 0, st>>>(B, node_id, node_neighbor_id, row_slot, s.tile_cnt);
-    GG_CHECK(cudaGetLastError());
-    int rc = gg::launch_exclusive_scan_i64(s.tile_cnt, n_tiles, nullptr, st);
+    int cur = 0;                                    // slots are < E
+    int rc = gg::number_and_group(gg::PairEntries{B, node_id, node_neighbor_id}, E, E - 1, row_slot, uniq_ids, n_unique, s.tile_cnt,
+                                  s.hist, s.key, s.val, st, &cur);
     if (rc) return rc;
-    gg::mc_number_kernel<<<n_tiles, gg::MC_THREADS, 0, st>>>(B, node_id, node_neighbor_id, s.tile_cnt, n_tiles, row_slot, uniq_ids,
-                                                              n_unique);
-    GG_CHECK(cudaGetLastError());
-    gg::mc_keys_kernel<<<n_tiles, gg::MC_THREADS, 0, st>>>(B, node_id, node_neighbor_id, row_slot, s.key[0], s.val[0]);
-    GG_CHECK(cudaGetLastError());
-    int bits = 1;                                   // slots are < E
-    while (bits < 31 && ((E - 1) >> bits) != 0) ++bits;
-    int cur = 0;
-    for (int shift = 0; shift < bits; shift += 8, cur ^= 1) {
-        gg::mc_hist_kernel<<<r_tiles, gg::MC_THREADS, 0, st>>>(E, s.key[cur], shift, r_tiles, s.hist);
-        GG_CHECK(cudaGetLastError());
-        rc = gg::launch_exclusive_scan_i64(s.hist, 256ll * r_tiles, nullptr, st);
-        if (rc) return rc;
-        gg::mc_scatter_kernel<<<r_tiles, gg::MC_THREADS, 0, st>>>(E, s.key[cur], s.val[cur], shift, r_tiles, s.hist, s.key[cur ^ 1],
-                                                                   s.val[cur ^ 1]);
-        GG_CHECK(cudaGetLastError());
-    }
     gg::mc_terms_kernel<<<grid, 256, 0, st>>>(mode, B, node_id, node_neighbor_id, emb, bias, ld, lambda, s.delta, s.key[cur],
                                                s.val[cur], s.off, s.terms);
     GG_CHECK(cudaGetLastError());
@@ -411,4 +560,46 @@ extern "C" int gg_pair_grad_ex(int32_t mode, int32_t n_pairs, int32_t batch_tota
         GG_CHECK(cudaGetLastError());
     }
     return 0;
+}
+
+extern "C" int gg_grad_merge_scratch_bytes(int32_t world, int32_t cap, int32_t ld, int64_t *bytes) {
+    GG_REQUIRE(bytes, "null pointer");
+    GG_REQUIRE(world >= 1 && cap >= 1, "world and cap must be >= 1");
+    GG_REQUIRE((int64_t)world * cap <= 2 * gg::MAX_PAIRS, "world * cap must be at most 2^31 - 8192 entries");
+    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    *bytes = (int64_t)gg::carve_merge(nullptr, (long long)world * cap).bytes;
+    return 0;
+}
+
+extern "C" int gg_grad_merge_ex(int32_t world, int32_t cap, int32_t ld, const float *gathered, int32_t *n_unique,
+                                int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot, void *scratch,
+                                int64_t scratch_bytes, int32_t flags, void *stream) {
+    GG_REQUIRE((flags & ~GG_GRAD_MULTI_CTA) == 0, "unknown flags");
+    GG_REQUIRE(world >= 1 && cap >= 1, "world and cap must be >= 1");
+    GG_REQUIRE((int64_t)world * cap <= 2 * gg::MAX_PAIRS, "world * cap must be at most 2^31 - 8192 entries");
+    if ((int64_t)world * cap <= 2 * GG_MAX_BATCH * 8 && !(flags & GG_GRAD_MULTI_CTA))
+        return gg_grad_merge(world, cap, ld, gathered, n_unique, uniq_ids, grad_rows, grad_bias, row_slot, stream);
+    GG_REQUIRE(gathered && n_unique && uniq_ids && grad_rows && grad_bias && row_slot, "null pointer");
+    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(world == 1 || cap % 2 == 0, "cap must be even when world > 1 (16-byte aligned blocks)");
+    GG_REQUIRE(((uintptr_t)gathered & 15) == 0, "gathered must be 16-byte aligned");
+    const int E = world * cap;
+    const gg::MergeScratch need = gg::carve_merge(nullptr, E);
+    GG_REQUIRE(scratch && scratch_bytes >= (int64_t)need.bytes, "scratch is null or smaller than gg_grad_merge_scratch_bytes");
+    GG_REQUIRE(((uintptr_t)scratch & 255) == 0, "scratch must be 256-byte aligned");
+    const gg::MergeScratch s = gg::carve_merge((char *)scratch, E);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int grid = gg::sm_count() * 8;
+    gg::mg_ids_kernel<<<grid, 256, 0, st>>>(E, cap, ld, gathered, s.ids, row_slot);
+    GG_CHECK(cudaGetLastError());
+    gg::mg_first_kernel<<<grid, 256, 0, st>>>(E, s.ids, row_slot);
+    GG_CHECK(cudaGetLastError());
+    int cur = 0;                                    // slots are < E, absent entries have key E
+    int rc = gg::number_and_group(gg::MergeEntries{s.ids}, E, E, row_slot, uniq_ids, n_unique, s.tile_cnt, s.hist, s.key, s.val, st,
+                                  &cur);
+    if (rc) return rc;
+    gg::mg_offsets_kernel<<<grid, 256, 0, st>>>(E, s.key[cur], s.off);
+    GG_CHECK(cudaGetLastError());
+    gg::mg_sums_kernel<<<grid, 256, 0, st>>>(cap, ld, gathered, n_unique, s.off, s.val[cur], grad_rows, grad_bias);
+    return gg::check_cuda(cudaGetLastError(), "merge sums launch");
 }

@@ -171,18 +171,20 @@ class PairModel:
         self.beta1_power, self.beta2_power = np.float32(b1p.value), np.float32(b2p.value)
         self.step_count += int(starts.size)
 
-    def _large_batch_buffers(self, B):
-        """Grow uniq_ids / grad_rows / grad_bias to 2B entries and the multi-CTA gradient's scratch to its size at B
-        (allocated on first use: models that never see a batch above GG_MAX_BATCH keep today's buffers)."""
+    def _large_batch_buffers(self, B, scratch_bytes=None):
+        """Grow uniq_ids / grad_rows / grad_bias to 2B entries and the scratch to `scratch_bytes` (default: the multi-CTA
+        gradient's size at B); allocated on first use: models that never see a batch above GG_MAX_BATCH keep today's buffers."""
         torch = self.torch
         if self.uniq_ids.numel() < 2 * B:
             self.uniq_ids = torch.zeros(2 * B, dtype=torch.int32, device=self.device)
             self.grad_rows = torch.zeros((2 * B, self.ld), dtype=torch.float32, device=self.device)
             self.grad_bias = torch.zeros(2 * B, dtype=torch.float32, device=self.device)
-        n = C.c_int64(0)
-        _cabi.check(self.lib.gg_pair_grad_scratch_bytes(int(B), self.ld, C.byref(n)), "gg_pair_grad_scratch_bytes")
-        if self._scratch is None or self._scratch.numel() < n.value:
-            self._scratch = torch.empty(n.value, dtype=torch.uint8, device=self.device)   # caching allocator: 512-byte aligned
+        if scratch_bytes is None:
+            n = C.c_int64(0)
+            _cabi.check(self.lib.gg_pair_grad_scratch_bytes(int(B), self.ld, C.byref(n)), "gg_pair_grad_scratch_bytes")
+            scratch_bytes = n.value
+        if self._scratch is None or self._scratch.numel() < scratch_bytes:
+            self._scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=self.device)   # caching allocator: 512-byte aligned
         return self._scratch
 
     def apply_adam(self):

@@ -5,11 +5,12 @@ graph and embeddings, takes a contiguous block of the root list, and -- because 
 by (root, walk, step) -- produces exactly the rows a single GPU would produce for those roots.  Rows are
 all-gathered so that every rank sees the same training set (the reference's lists, in root order).
 
-Updates are data parallel: every rank scores its slice of the 64-pair batch (K2), ONE collective per step
-exchanges the compact gradients (ids + summed rows; a few KB, latency bound, NVLS-friendly), every rank merges
-them in the same rank-major order (gg_grad_merge) and applies the same K3 Adam sweep, so replicas stay
-bit-identical without broadcasting parameters.  The step lives in the C library (csrc/comm.cu: gg_dp_step,
-gg_dp_train_steps) with a library-owned NCCL communicator; torch.distributed only carries the 128-byte unique id.
+Updates are data parallel: every rank scores its slice of the mini-batch (K2), ONE collective per step
+exchanges the compact gradients (ids + summed rows; a few KB at 64 pairs, latency bound, NVLS-friendly), every rank
+merges them in the same rank-major order (gg_grad_merge; gg_grad_merge_ex, multi-CTA, above GG_MAX_BATCH pairs) and
+applies the same K3 Adam sweep, so replicas stay bit-identical without broadcasting parameters.  The step lives in
+the C library (csrc/comm.cu: gg_dp_step, gg_dp_train_steps, and their _ex forms for any batch size) with a
+library-owned NCCL communicator; torch.distributed only carries the 128-byte unique id.
 """
 import ctypes as C
 
@@ -91,12 +92,6 @@ def connect_peer_memory(comm, capacity_floats, group=None):
     _cabi.check(lib.gg_comm_p2p_connect(comm, C.create_string_buffer(raw, 64 * world)), "gg_comm_p2p_connect")
 
 
-def _check_batch(B):
-    """The data-parallel gradient, exchange and merge are one-CTA kernels: refuse larger batches before communicating."""
-    if B > MAX_BATCH:
-        raise ValueError("data-parallel steps take at most GG_MAX_BATCH=%d pairs per batch, not %d" % (MAX_BATCH, B))
-
-
 class DataParallelStep:
     """Data-parallel replacement for PairModel.step / train_steps: same arguments (the WHOLE mini-batch, identical on
     every rank).  The step -- gradient of this rank's rows, ONE ncclAllGather of the compact gradients, rank-major merge,
@@ -104,6 +99,7 @@ class DataParallelStep:
 
     _comm = None        # one library-owned communicator per process
     _p2p_capacity = 0   # floats of the peer-memory exchange buffer (0: not connected)
+    transport = None    # "nccl" or "p2p" once use() has run
 
     def __init__(self, model, group=None, transport="nccl"):
         import torch
@@ -128,6 +124,19 @@ class DataParallelStep:
             DataParallelStep._p2p_capacity = cap_floats
         self.transport = transport
 
+    def _check_batch(self, B):
+        """Above GG_MAX_BATCH pairs only the NCCL transport has a path (multi-CTA gradient and merge); the peer-memory
+        exchange is sized for small batches and fused into a one-CTA kernel.  Refuse before communicating."""
+        if B > MAX_BATCH and self.transport != "nccl":
+            raise ValueError("data-parallel steps above GG_MAX_BATCH=%d pairs per batch (here %d) need the nccl transport, not %s"
+                             % (MAX_BATCH, B, self.transport))
+
+    def _large_batch_scratch(self, B):
+        """Model gradient buffers of 2B entries and the scratch of gg_dp_scratch_bytes (shared with PairModel's)."""
+        m, n = self.model, C.c_int64(0)
+        _cabi.check(self.lib.gg_dp_scratch_bytes(self.world, int(B), m.ld, C.byref(n)), "gg_dp_scratch_bytes")
+        return m._large_batch_buffers(int(B), n.value)
+
     def _select(self):
         _cabi.check(self.lib.gg_comm_use_p2p(self.comm, 1 if self.transport == "p2p" else 0), "gg_comm_use_p2p")
 
@@ -146,11 +155,22 @@ class DataParallelStep:
         B = int(i.shape[0])
         if B == 0:
             return
-        _check_batch(B)
+        self._check_batch(B)
         cap = 2 * (-(-B // self.world))
         local, gathered = self._buffers(cap)
         self._select()
         f = lambda x: C.c_float(float(x))
+        if B > MAX_BATCH:
+            scratch = self._large_batch_scratch(B)
+            _cabi.check(self.lib.gg_dp_step_ex(self.comm, m._step_mode, B, ptr(i), ptr(j), ptr(a), m.n_node, m.ld, ptr(m.emb),
+                                               ptr(m.m_emb), ptr(m.v_emb), ptr(m.bias_t), ptr(m.m_bias), ptr(m.v_bias), f(m.lam),
+                                               ptr(local), ptr(gathered), cap, ptr(m.n_unique), ptr(m.uniq_ids), ptr(m.grad_rows),
+                                               ptr(m.grad_bias), ptr(m.row_slot), f(m.lr_t()), f(m.beta1), f(m.beta2), f(m.eps),
+                                               ptr(scratch), scratch.numel(), 0, m._stream()), "gg_dp_step_ex")
+            m.beta1_power = np.float32(m.beta1_power * m.beta1)
+            m.beta2_power = np.float32(m.beta2_power * m.beta2)
+            m.step_count += 1
+            return
         _cabi.check(self.lib.gg_dp_step(self.comm, m._step_mode, B, ptr(i), ptr(j), ptr(a), m.n_node, m.ld, ptr(m.emb), ptr(m.m_emb),
                                         ptr(m.v_emb), ptr(m.bias_t), ptr(m.m_bias), ptr(m.v_bias), f(m.lam), ptr(local), ptr(gathered),
                                         cap, ptr(m.n_unique), ptr(m.uniq_ids), ptr(m.grad_rows), ptr(m.grad_bias), ptr(m.row_slot),
@@ -161,7 +181,7 @@ class DataParallelStep:
 
     def train_steps(self, node_id, node_neighbor_id, aux, start_list, batch_size):
         """All steps of one inner epoch (graph_gan.py:149-157 / 168-176) enqueued from C, one collective each."""
-        _check_batch(batch_size)
+        self._check_batch(batch_size)
         m = self.model
         i, j, a = m._dev_i32(node_id), m._dev_i32(node_neighbor_id), m._dev_f32(aux)
         starts = np.ascontiguousarray(np.asarray(start_list, np.int64))
@@ -172,12 +192,22 @@ class DataParallelStep:
         self._select()
         f = lambda x: C.c_float(float(x))
         b1p, b2p = f(m.beta1_power), f(m.beta2_power)
-        _cabi.check(self.lib.gg_dp_train_steps(self.comm, m._step_mode, int(i.shape[0]), starts.ctypes.data_as(C.c_void_p),
-                                               int(starts.size), int(batch_size), ptr(i), ptr(j), ptr(a), m.n_node, m.ld,
-                                               ptr(m.emb), ptr(m.m_emb), ptr(m.v_emb), ptr(m.bias_t), ptr(m.m_bias), ptr(m.v_bias),
-                                               f(m.lam), ptr(local), ptr(gathered), cap, ptr(m.n_unique), ptr(m.uniq_ids),
-                                               ptr(m.grad_rows), ptr(m.grad_bias), ptr(m.row_slot), f(m.lr), f(m.beta1), f(m.beta2),
-                                               f(m.eps), C.byref(b1p), C.byref(b2p), m._stream()), "gg_dp_train_steps")
+        if batch_size > MAX_BATCH:
+            scratch = self._large_batch_scratch(batch_size)
+            _cabi.check(self.lib.gg_dp_train_steps_ex(self.comm, m._step_mode, int(i.shape[0]), starts.ctypes.data_as(C.c_void_p),
+                                                      int(starts.size), int(batch_size), ptr(i), ptr(j), ptr(a), m.n_node, m.ld,
+                                                      ptr(m.emb), ptr(m.m_emb), ptr(m.v_emb), ptr(m.bias_t), ptr(m.m_bias),
+                                                      ptr(m.v_bias), f(m.lam), ptr(local), ptr(gathered), cap, ptr(m.n_unique),
+                                                      ptr(m.uniq_ids), ptr(m.grad_rows), ptr(m.grad_bias), ptr(m.row_slot), f(m.lr),
+                                                      f(m.beta1), f(m.beta2), f(m.eps), C.byref(b1p), C.byref(b2p), ptr(scratch),
+                                                      scratch.numel(), 0, m._stream()), "gg_dp_train_steps_ex")
+        else:
+            _cabi.check(self.lib.gg_dp_train_steps(self.comm, m._step_mode, int(i.shape[0]), starts.ctypes.data_as(C.c_void_p),
+                                                   int(starts.size), int(batch_size), ptr(i), ptr(j), ptr(a), m.n_node, m.ld,
+                                                   ptr(m.emb), ptr(m.m_emb), ptr(m.v_emb), ptr(m.bias_t), ptr(m.m_bias), ptr(m.v_bias),
+                                                   f(m.lam), ptr(local), ptr(gathered), cap, ptr(m.n_unique), ptr(m.uniq_ids),
+                                                   ptr(m.grad_rows), ptr(m.grad_bias), ptr(m.row_slot), f(m.lr), f(m.beta1), f(m.beta2),
+                                                   f(m.eps), C.byref(b1p), C.byref(b2p), m._stream()), "gg_dp_train_steps")
         self._keep = (i, j, a)
         m.beta1_power, m.beta2_power = np.float32(b1p.value), np.float32(b2p.value)
         m.step_count += int(starts.size)

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 4
+#define GG_ABI_VERSION 5
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -245,6 +245,18 @@ int gg_pair_grad_ex(int32_t mode, int32_t n_pairs, int32_t batch_total, const in
 int64_t gg_grad_buf_floats(int32_t cap, int32_t ld);
 int gg_grad_merge(int32_t world, int32_t cap, int32_t ld, const float *gathered, int32_t *n_unique,
                   int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot, void *stream);
+/* The same merge for any number of entries (world * cap <= 2^31 - 8192; csrc/grad_multi.cu): outputs identical, bit for bit,
+ * to gg_grad_merge on every input gg_grad_merge accepts.  Entry t = r * cap + s exists for s < the n_unique word of rank
+ * r's block; slots are numbered in order of first occurrence over t, and every coordinate of a slot is one +0-started
+ * round-to-nearest add chain over the slot's entries in rank order.  row_slot may still hold this rank's local slots on
+ * entry (as gg_pair_grad[_ex] leaves them).  Up to world * cap = 16384 entries without flags it runs gg_grad_merge's
+ * one-CTA kernel; otherwise a multi-CTA path (GG_GRAD_MULTI_CTA forces it) that needs `scratch` (device, 256-byte
+ * aligned, at least gg_grad_merge_scratch_bytes(world, cap, ld) bytes, linear in world * cap), cap even when world > 1,
+ * and `gathered` 16-byte aligned.  gg_grad_merge_scratch_bytes is a host-only size computation. */
+int gg_grad_merge_scratch_bytes(int32_t world, int32_t cap, int32_t ld, int64_t *bytes);
+int gg_grad_merge_ex(int32_t world, int32_t cap, int32_t ld, const float *gathered, int32_t *n_unique,
+                     int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot, void *scratch,
+                     int64_t scratch_bytes, int32_t flags, void *stream);
 
 /* ------------------------------------------------------------------------------------------
  * Data-parallel optimizer step with its collective inside the library (csrc/comm.cu).  N replicas of the
@@ -284,6 +296,30 @@ int gg_dp_train_steps(void *comm, int32_t mode, int64_t n_rows, const int64_t *s
                       int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot,
                       float lr, float beta1, float beta2, float eps, float *beta1_power, float *beta2_power,
                       void *stream);
+/* The data-parallel step for any batch size (1 .. 2^30 - 4096 pairs).  Up to GG_MAX_BATCH pairs without flags,
+ * gg_dp_step_ex / gg_dp_train_steps_ex are gg_dp_step / gg_dp_train_steps.  Otherwise every rank computes its slice
+ * with gg_pair_grad_ex (batch_total = n_pairs; one CTA up to GG_MAX_BATCH pairs per slice, multi-CTA above), runs the
+ * same single ncclAllGather and merges with the multi-CTA gg_grad_merge_ex.  GG_GRAD_MULTI_CTA forces the multi-CTA
+ * gradient and merge at any size.  uniq_ids / grad_rows / grad_bias hold 2 * n_pairs entries; scratch: device, 256-byte
+ * aligned, at least gg_dp_scratch_bytes(world, n_pairs, ld) bytes with cap = 2 * ceil(n_pairs / world) (a larger cap
+ * needs gg_grad_merge_scratch_bytes(world, cap, ld)); gg_dp_scratch_bytes is host-only, the larger of the slice
+ * gradient's and the merge's scratch, which run one after the other and share the buffer.  The peer-memory transport
+ * stays limited to GG_MAX_BATCH pairs: with it switched on, larger batches (or flags) return an error.
+ * gg_dp_train_steps_ex lays out each step's blocks with cap = 2 * ceil(rows of the step / world). */
+int gg_dp_scratch_bytes(int32_t world, int32_t n_pairs, int32_t ld, int64_t *bytes);
+int gg_dp_step_ex(void *comm, int32_t mode, int32_t n_pairs, const int32_t *node_id, const int32_t *node_neighbor_id,
+                  const float *aux, int64_t n_node, int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias,
+                  float *m_bias, float *v_bias, float lambda, float *local_buf, float *gathered_buf, int32_t cap,
+                  int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot,
+                  float lr_t, float beta1, float beta2, float eps, void *scratch, int64_t scratch_bytes, int32_t flags,
+                  void *stream);
+int gg_dp_train_steps_ex(void *comm, int32_t mode, int64_t n_rows, const int64_t *start_list, int64_t n_starts,
+                         int32_t batch_size, const int32_t *node_id, const int32_t *node_neighbor_id, const float *aux,
+                         int64_t n_node, int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias, float *m_bias,
+                         float *v_bias, float lambda, float *local_buf, float *gathered_buf, int32_t cap,
+                         int32_t *n_unique, int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot,
+                         float lr, float beta1, float beta2, float eps, float *beta1_power, float *beta2_power,
+                         void *scratch, int64_t scratch_bytes, int32_t flags, void *stream);
 
 /* K3: TF1.8 AdamOptimizer sparse apply == dense decay (generator.py:30-31,
  * discriminator.py:31-32): m <- b1*m (+ (1-b1) g on touched rows), v likewise, then for ALL
