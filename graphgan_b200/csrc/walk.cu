@@ -412,24 +412,33 @@ struct FlatView {
     int4 *list[2];         // [W] walks that execute step s next, as records (walk, node it stands on, node it came from,
                            //     root slot): list[s & 1] -- one 16-byte load gives a kernel everything about the walk
     int4 *tail;            // [W] walks the persistent kernel finishes (after the last level-synchronous step), same records
-    int *hub;              // [W] per level: items (indices into the level's list) that stand on a score-cached node
+    int *hub;              // [W] per level: items (indices into the level's list) that stand on a score-cached node; on a
+                           //     level that groups them (SHARE_HUB): the records that own a distinct hub key
     int *item_n;           // [W] per item: candidate-list length | father flag << 30 (0: nothing left to do for the item)
     int *pool_ids;         // [W * stride] per item: its candidate ids
     unsigned *ctr;         // counters: [0] tail length; level s: [1 + 4 s + {0: items, 1: hub items, 2: distinct keys of a
-                           //     shared level, 3: work queue}]
+                           //     shared level that are not score-cached, 3: work queue}]; after them, level s of a level that
+                           //     groups hub items: [FLAT_CTR_WORDS + 3 s + {0: hub owners, 1: hub work items, 2: members placed}]
     int stride;            // pool entries per item (>= hub_threshold: a node below the threshold has fewer neighbours)
     int steps;             // level-synchronous steps 1 .. steps
     // shared levels (SHARE_LEVELS): one candidate list + CDF per distinct (root slot, node), every walk on it draws from it
     unsigned long long *keys;   // [tbl_mask + 1] open-addressing table of slot * n_node + node (empty: ~0)
     int *owner;            // [tbl_mask + 1] per table slot: the record that inserted the key (its item owns the list)
-    int *rec_slot;         // [W] per record: its table slot (-1: a hub item, run per walk)
+    int *rec_slot;         // [W] per record: its table slot (-1: a hub item, run per walk; -2 - slot: a grouped hub item)
     int *uniq;             // [W] the level's distinct keys that are not score-cached, as the records that own them
     double *pool_cdf;      // [W * (stride + 1)] per owning item: its un-normalised CDF and the total (cdf_store_raw)
     unsigned long long tbl_mask;
+    // hub groups (SHARE_HUB): the walks of a shared level on one score-cached (root slot, node) are drawn by one warp
+    unsigned *gcnt;        // [tbl_mask + 1] per table slot: walks on the hub key
+    unsigned *gpos;        // [tbl_mask + 1] per table slot: the next free place of the key's range of hub_rec
+    int *hub_rec;          // [W] the hub records, each group contiguous
+    int4 *hub_work;        // [W] work items: (owner record, first place in hub_rec, members, 0), <= HUB_GROUP_MAX members
 };
 constexpr int FLAT_MAX_STEPS = 14;
 constexpr int FLAT_CTR_WORDS = 1 + 4 * (FLAT_MAX_STEPS + 2);
+constexpr int FLAT_CTR_ALL = FLAT_CTR_WORDS + 3 * (FLAT_MAX_STEPS + 2);
 #define GG_FCTR(fv, s, k) ((fv).ctr + 1 + 4 * (s) + (k))
+#define GG_FCTR_HUB(fv, s, k) ((fv).ctr + FLAT_CTR_WORDS + 3 * (s) + (k))
 // the record list of level s (a select: a run-time index into the kernel parameter would copy it to local memory)
 __device__ __forceinline__ int4 *level_list(const FlatView &fv, int s) { return (s & 1) ? fv.list[1] : fv.list[0]; }
 
@@ -443,6 +452,20 @@ constexpr unsigned SHARE_LEVELS = (unsigned)(GG_SHARE_LEVELS) & ~3u;
 __host__ __device__ constexpr bool level_shared(int s) { return s < 32 && ((SHARE_LEVELS >> s) & 1u); }
 // does any of the levels 1 .. steps share?
 inline bool any_level_shared(int steps) { return steps >= 2 && (SHARE_LEVELS & ((steps >= 31 ? ~0u : ((2u << steps) - 1u)))) != 0; }
+
+// On a shared level, the walks that stand on one score-cached (hub) node of one root are a group: one warp builds the
+// list once and draws every walk of the group from it while the list is still in its score buffer (nothing is stored).
+// 0 = hub walks run per walk, as on a level that does not share.  A group of more than HUB_GROUP_MAX walks is split into
+// work items that each build the list, so that no single item is the launch's tail.
+#ifndef GG_SHARE_HUB
+#define GG_SHARE_HUB 1
+#endif
+#ifndef GG_HUB_GROUP_MAX
+#define GG_HUB_GROUP_MAX 128
+#endif
+constexpr bool SHARE_HUB = GG_SHARE_HUB != 0;
+constexpr int HUB_GROUP_MAX = GG_HUB_GROUP_MAX;
+static_assert(HUB_GROUP_MAX > 0 && HUB_GROUP_MAX % 32 == 0, "hub work items are whole warps of walks");
 
 template <int CPL>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) walk_kernel(const __grid_constant__ gg_walk_desc d,
@@ -658,9 +681,12 @@ __global__ void __launch_bounds__(256) flat_start_kernel(const __grid_constant__
 }
 
 // ---- shared levels: (1) flat_dedupe_kernel, thread per record: the record's key (root slot, node) goes into the level's
-// hash table; the record that inserts a key owns its item (candidate list + CDF); score-cached (hub) nodes go to the hub
-// list as in flat_enum_kernel and run per walk.  (2) flat_enum_kernel<true> + flat_choose_kernel<C, true>: the owners' lists
-// and their CDFs.  (3) flat_draw_kernel, thread per record: the walk's uniform inverts its item's CDF.
+// hash table; the record that inserts a key owns its item (candidate list + CDF).  A key on a score-cached (hub) node is a
+// hub group (SHARE_HUB): its owner goes to the hub list, and flat_hub_reserve_kernel + flat_hub_fill_kernel lay out the
+// group's records contiguously (without SHARE_HUB, hub records go to the hub list one each and run per walk).
+// (2) flat_enum_kernel<true> + flat_choose_kernel<C, true>: the owners' lists and their CDFs; a hub group's warp builds
+// its list and draws all its walks at once.  (3) flat_draw_kernel, thread per record: the walk's uniform inverts its
+// item's CDF (hub records were drawn in step 2).
 __device__ __forceinline__ unsigned long long share_hash(unsigned long long key, unsigned long long mask) {
     return ((key * 0x9E3779B97F4A7C15ull) >> 20) & mask;
 }
@@ -688,7 +714,7 @@ __global__ void __launch_bounds__(256) flat_dedupe_kernel(const __grid_constant_
         const int cur = rec.y, slot = rec.w;
         hub = d.edge_score && (d.indptr[cur + 1] - d.indptr[cur]) >= d.hub_threshold;
         int h = -1;
-        if (!hub) {
+        if (!hub || SHARE_HUB) {
             const unsigned long long key = (unsigned long long)slot * (unsigned long long)d.n_node + (unsigned long long)cur;
             unsigned long long p = share_hash(key, fv.tbl_mask);
             for (;;) {                                     // linear probing; the table has >= 2 slots per record
@@ -698,12 +724,69 @@ __global__ void __launch_bounds__(256) flat_dedupe_kernel(const __grid_constant_
                 p = (p + 1) & fv.tbl_mask;
             }
             h = (int)p;
+            if (hub) {                                     // a member of the hub group: counted, and negative for flat_draw_kernel
+                atomicAdd(fv.gcnt + p, 1u);
+                h = -2 - h;
+            }
         }
         fv.rec_slot[i] = h;
     }
     const int item = (int)i;
-    warp_append(hub, fv.hub, GG_FCTR(fv, s, 1), item, lane);
-    warp_append(owner, fv.uniq, GG_FCTR(fv, s, 2), item, lane);
+    if (SHARE_HUB) {
+        const unsigned mk = __ballot_sync(FULL, hub);
+        if (lane == 0 && mk) atomicAdd(GG_FCTR(fv, s, 1), (unsigned)__popc(mk));
+        warp_append(hub && owner, fv.hub, GG_FCTR_HUB(fv, s, 0), item, lane);
+    } else {
+        warp_append(hub, fv.hub, GG_FCTR(fv, s, 1), item, lane);
+    }
+    warp_append(owner && !hub, fv.uniq, GG_FCTR(fv, s, 2), item, lane);
+}
+
+// exclusive offset of this lane's `v` in a range of sum(v) reserved on `cnt` with one atomic per warp
+__device__ __forceinline__ unsigned warp_reserve(unsigned v, unsigned *cnt, int lane) {
+    unsigned incl = v;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const unsigned x = __shfl_up_sync(FULL, incl, off);
+        if (lane >= off) incl += x;
+    }
+    unsigned base = 0;
+    if (lane == 31 && incl) base = atomicAdd(cnt, incl);
+    return __shfl_sync(FULL, base, 31) + incl - v;
+}
+
+// thread per hub owner: its group's range of hub_rec, and the group's work items (at most HUB_GROUP_MAX walks each)
+__global__ void __launch_bounds__(256) flat_hub_reserve_kernel(const FlatView fv, const int s) {
+    const unsigned j = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31;
+    const unsigned nO = *GG_FCTR_HUB(fv, s, 0);
+    if (blockIdx.x * blockDim.x >= nO) return;             // warp-uniform below
+    int orec = 0;
+    unsigned p = 0, cnt = 0, nw = 0;
+    if (j < nO) {
+        orec = fv.hub[j];
+        p = (unsigned)(-2 - fv.rec_slot[orec]);
+        cnt = fv.gcnt[p];
+        nw = (cnt + HUB_GROUP_MAX - 1) / HUB_GROUP_MAX;
+    }
+    const unsigned base = warp_reserve(cnt, GG_FCTR_HUB(fv, s, 2), lane);
+    const unsigned it = warp_reserve(nw, GG_FCTR_HUB(fv, s, 1), lane);
+    if (j < nO) {
+        fv.gpos[p] = base;
+        for (unsigned q = 0; q < nw; ++q) {
+            const unsigned first = q * HUB_GROUP_MAX;
+            fv.hub_work[it + q] = make_int4(orec, (int)(base + first), (int)min(cnt - first, (unsigned)HUB_GROUP_MAX), 0);
+        }
+    }
+}
+
+// thread per record: a hub record takes the next place of its group's range (the order within a group is free: every
+// walk draws its own uniform)
+__global__ void __launch_bounds__(256) flat_hub_fill_kernel(const FlatView fv, const int s) {
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= *GG_FCTR(fv, s, 0)) return;
+    const int h = fv.rec_slot[i];
+    if (h <= -2) fv.hub_rec[atomicAdd(fv.gpos + (-2 - h), 1u)] = (int)i;
 }
 
 __global__ void __launch_bounds__(256) flat_draw_kernel(const __grid_constant__ gg_walk_desc d, const FlatView fv, const int s) {
@@ -831,7 +914,9 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose
     int *g_ids = reinterpret_cast<int *>(d.scratch) + (size_t)gw * 2 * (size_t)d.max_cand;
     float *g_sc = reinterpret_cast<float *>(g_ids + d.max_cand);
     const int4 *A = level_list(fv, s);
-    const unsigned nA = SHARED ? *GG_FCTR(fv, s, 2) : *GG_FCTR(fv, s, 0), nH = *GG_FCTR(fv, s, 1);
+    constexpr bool GROUPS = SHARED && SHARE_HUB;
+    const unsigned nA = SHARED ? *GG_FCTR(fv, s, 2) : *GG_FCTR(fv, s, 0);
+    const unsigned nH = GROUPS ? *GG_FCTR_HUB(fv, s, 1) : *GG_FCTR(fv, s, 1);
     const uint32_t k0 = (uint32_t)d.seed, k1 = (uint32_t)(d.seed >> 32);
     unsigned long long raw_steps = 0, raw_suml = 0, overflow = 0, rows_gathered = 0;
     unsigned int cyc[7] = {0, 0, 0, 0, 0, 0, 0};
@@ -846,6 +931,55 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose
         j = __shfl_sync(FULL, j, 0);
         if (j >= n_pulls) break;
         const bool hub_item = j < nH;
+        if (GROUPS && hub_item) {
+            // ---- a hub group (or a part of one): the walks of one root on one score-cached node.  From step 2 on their
+            // list is [tree father] + children(cur) for all of them; it is built and prepared once, then every walk
+            // inverts it with its own uniform: lane t holds the walk of the t-th draw of each round of 32
+            const int4 hw = fv.hub_work[j];
+            const int4 orec = A[hw.x];
+            const int cur = orec.y, prev = orec.z, slot = orec.w;
+            const int root = d.roots[slot];
+            const long long wp = __ldg(d.walk_ptr + slot);
+            int w_lane = (lane < hw.z) ? A[fv.hub_rec[hw.y + lane]].x : 0;      // in flight while the list is built
+            const uint32_t *tb = d.tree_bits + (size_t)slot * (size_t)d.tree_words;
+            int n; float m; int *ids; float *sc;
+            build_list<CPL, UNR>(d, tb, cur, prev, true, s_ids, s_sc, g_ids, g_sc, lane, n, m, ids, sc, rows_gathered, cyc, stg);
+            double *tiles = sc != s_sc ? reinterpret_cast<double *>(s_sc) : nullptr;
+            ListCdf cdf;
+            if (n >= 2) cdf_prepare(sc, n, m, lane, tiles, cdf);
+            unsigned long long ov = 0;
+            for (int q0 = 0; q0 < hw.z; q0 += 32) {
+                if (q0) w_lane = (q0 + lane < hw.z) ? A[fv.hub_rec[hw.y + q0 + lane]].x : 0;
+                const int nq = min(32, hw.z - q0);
+                const bool mine = lane < nq;
+                int idx = 0;                               // n == 1: index 0 for every walk (see build_list)
+                if (n >= 2) {
+                    // each lane draws the uniform of its own walk; the inversions (warp-wide) run one after the other
+                    uint32_t a, b;
+                    philox4x32_10((uint32_t)root, (uint32_t)(w_lane - wp), (uint32_t)s, d.pass_tag, k0, k1, a, b);
+                    const double u_lane = u53(a, b);
+                    for (int t = 0; t < nq; ++t) {
+                        const int it = cdf_draw(sc, n, cdf, __shfl_sync(FULL, u_lane, t), lane, tiles);
+                        if (lane == t) idx = it;
+                    }
+                }
+                bool go_on = false;
+                int4 next = make_int4(0, 0, 0, 0);
+                if (mine && n == 0) flat_void(d, s, w_lane);
+                if (mine && n > 0) {
+                    const int nxt = ids[idx];
+                    go_on = flat_record_choice(d, s, w_lane, cur, n, idx, nxt, true, ov);
+                    next = make_int4(w_lane, nxt, cur, slot);
+                }
+                if (s < fv.steps) warp_append(go_on, level_list(fv, s + 1), GG_FCTR(fv, s + 1, 0), next, lane);
+                else warp_append(go_on, fv.tail, fv.ctr, next, lane);
+                if (lane == 0 && n > 0) { raw_steps += (unsigned)nq; raw_suml += (unsigned)nq * (unsigned)n; }
+            }
+            const unsigned ovw = __reduce_add_sync(FULL, (unsigned)ov);
+            if (lane == 0) overflow += ovw;
+            __syncwarp();                                  // every lane is done with ids / sc before the next pull
+            continue;
+        }
         unsigned p = hub_item ? 0u : (j - nH) * FLAT_CHUNK;
         const unsigned p_end = hub_item ? 1u : ((p + FLAT_CHUNK < nA) ? p + FLAT_CHUNK : nA);
         unsigned i_next = hub_item ? (unsigned)fv.hub[j] : (SHARED ? (unsigned)fv.uniq[p] : p);
@@ -923,14 +1057,17 @@ size_t flat_layout(void *buf, long long n_walks, int hub_threshold, int steps, F
         off += (bytes + 255) & ~(size_t)255;
         return p;
     };
-    unsigned *ctr = (unsigned *)take(sizeof(unsigned) * FLAT_CTR_WORDS);
+    unsigned *ctr = (unsigned *)take(sizeof(unsigned) * FLAT_CTR_ALL);
     int4 *l0 = (int4 *)take(16 * W), *l1 = (int4 *)take(16 * W), *tail = (int4 *)take(16 * W);
     int *hub = (int *)take(4 * W), *item_n = (int *)take(4 * W);
     int *pool = (int *)take(4 * W * (size_t)stride);
-    // shared levels: a table of >= 2 slots per record (W = 322 k: 2^20 slots, 12 MB), the owners' CDF slab (332 MB)
+    // shared levels: a table of >= 2 slots per record (W = 322 k: 2^20 slots, 12 MB), the owners' CDF slab (332 MB); hub
+    // groups: a count and a place per table slot (8 MB), the grouped records and the work items (6.4 MB)
     unsigned long long cap = 0;
     unsigned long long *keys = nullptr;
-    int *owner = nullptr, *rec_slot = nullptr, *uniq = nullptr;
+    int *owner = nullptr, *rec_slot = nullptr, *uniq = nullptr, *hub_rec = nullptr;
+    unsigned *gcnt = nullptr, *gpos = nullptr;
+    int4 *hub_work = nullptr;
     double *cdf = nullptr;
     if (any_level_shared(steps)) {
         cap = 1;
@@ -940,12 +1077,19 @@ size_t flat_layout(void *buf, long long n_walks, int hub_threshold, int steps, F
         rec_slot = (int *)take(4 * W);
         uniq = (int *)take(4 * W);
         cdf = (double *)take(8 * W * (size_t)(stride + 1));
+        if (SHARE_HUB) {
+            gcnt = (unsigned *)take(4 * cap);
+            gpos = (unsigned *)take(4 * cap);
+            hub_rec = (int *)take(4 * W);
+            hub_work = (int4 *)take(16 * W);
+        }
     }
     if (fv) {
         fv->ctr = ctr; fv->list[0] = l0; fv->list[1] = l1; fv->tail = tail; fv->hub = hub;
         fv->item_n = item_n; fv->pool_ids = pool; fv->stride = stride; fv->steps = steps;
         fv->keys = keys; fv->owner = owner; fv->rec_slot = rec_slot; fv->uniq = uniq; fv->pool_cdf = cdf;
         fv->tbl_mask = cap ? cap - 1 : 0;
+        fv->gcnt = gcnt; fv->gpos = gpos; fv->hub_rec = hub_rec; fv->hub_work = hub_work;
     }
     return off;
 }
@@ -1196,7 +1340,7 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
             GG_REQUIRE(d.flat_buf && d.flat_bytes >= (int64_t)gg::flat_layout(nullptr, d.n_walks, d.hub_threshold, d.flat_steps, nullptr),
                        "flat_buf too small (gg_walk_flat_bytes)");
             gg::flat_layout(d.flat_buf, d.n_walks, d.hub_threshold, d.flat_steps, &fv);
-            GG_CHECK(cudaMemsetAsync(fv.ctr, 0, sizeof(unsigned) * gg::FLAT_CTR_WORDS, st));
+            GG_CHECK(cudaMemsetAsync(fv.ctr, 0, sizeof(unsigned) * gg::FLAT_CTR_ALL, st));
             gg::flat_start_kernel<<<(unsigned)((d.n_walks + 255) / 256), 256, 0, st>>>(d, fv);
             GG_CHECK(cudaGetLastError());
             const int enum_ctas = gg::sm_count() * 8;
@@ -1206,8 +1350,15 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
                 const bool shared = gg::level_shared(s);
                 if (shared) {
                     GG_CHECK(cudaMemsetAsync(fv.keys, 0xff, sizeof(unsigned long long) * (size_t)(fv.tbl_mask + 1), st));
+                    if (gg::SHARE_HUB) GG_CHECK(cudaMemsetAsync(fv.gcnt, 0, sizeof(unsigned) * (size_t)(fv.tbl_mask + 1), st));
                     gg::flat_dedupe_kernel<<<rec_ctas, 256, 0, st>>>(d, fv, s);
                     GG_CHECK(cudaGetLastError());
+                    if (gg::SHARE_HUB) {
+                        gg::flat_hub_reserve_kernel<<<rec_ctas, 256, 0, st>>>(fv, s);
+                        GG_CHECK(cudaGetLastError());
+                        gg::flat_hub_fill_kernel<<<rec_ctas, 256, 0, st>>>(fv, s);
+                        GG_CHECK(cudaGetLastError());
+                    }
                     gg::flat_enum_kernel<true><<<enum_ctas, gg::FLAT_ENUM_WARPS * 32, 0, st>>>(d, fv, s);
                 } else {
                     gg::flat_enum_kernel<false><<<enum_ctas, gg::FLAT_ENUM_WARPS * 32, 0, st>>>(d, fv, s);

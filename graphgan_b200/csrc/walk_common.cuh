@@ -221,7 +221,6 @@ __device__ __forceinline__ int cdf_pick(const float *sc, int n, float S, double 
     return cdf_pick_from(sc, n, S, total, u, lane, t_hit, before);
 }
 
-// softmax + CDF + draw over sc[0..n) given its max m (== ggo_choose).  All lanes return the index.
 // Long lists (global scratch): running total after EVERY tile goes to `tiles` (the warp's idle shared score buffer
 // viewed as doubles), so the draw can locate its tile among hundreds without a linear scan.
 __device__ __forceinline__ double cdf_total_tiles(const float *sc, int n, float S, int lane, double *tiles) {
@@ -258,13 +257,49 @@ __device__ __forceinline__ int cdf_pick_tiles(const float *sc, int n, float S, d
     return n - 1;
 }
 
+// One tile (n <= 32, the common case): S = 0 + T_0 = T_0, total = 0 + scan_31 = scan_31 and the carry of the draw is 0, so
+// the canonical sequence collapses to ONE scan and ONE division per lane -- the same floats, bit for bit.  Returns the
+// lane's inclusive scan x; the draw for u is the first lane with x / total > u.
+__device__ __forceinline__ double tile1_cdf(const float *sc, int n, float m, int lane, double &total) {
+    const float e = (lane < n) ? exp_c(__fsub_rn(sc[lane], m)) : 0.0f;
+    const float S = warp_sum_butterfly(e);
+    const double x = warp_scan_ks((double)__fdiv_rn(e, S), lane);
+    total = __shfl_sync(FULL, x, 31);
+    return x;
+}
+__device__ __forceinline__ int tile1_pick(double x, double total, int n, double u, int lane) {
+    const unsigned hit = __ballot_sync(FULL, (lane < n) && (__ddiv_rn(x, total) > u));
+    return hit ? __ffs(hit) - 1 : n - 1;
+}
+
+// A list's softmax + CDF, built once by cdf_prepare; cdf_draw then inverts it for as many uniforms as needed (it does
+// not write sc).  Both run the passes choose_index runs, so a draw is the same bits whether or not other draws share
+// the list.
+struct ListCdf {
+    float S;           // canonical softmax denominator
+    double total;      // the CDF's total
+    double car[2];     // n <= 32: car[0] = the lane's scan (tile1_cdf); else cdf_total's running totals
+};
+
 // lists longer than the shared score buffer (global scratch): rare, so kept out of line and modestly unrolled -- the
-// walk kernel's instruction footprint is what its warps stall on otherwise (ncu: "no instruction")
+// walk kernel's instruction footprint is what its warps stall on otherwise (ncu: "no instruction").  With `tiles`, the
+// running total after EVERY tile goes to the (idle) shared score buffer: the draw finds its tile among hundreds directly.
+__device__ __forceinline__ bool long_uses_tiles(int n, const double *tiles) { return tiles && ((n + 31) >> 5) <= SC_CAP / 2; }
+static __device__ __noinline__ void cdf_prepare_long(float *sc, int n, float m, int lane, double *tiles, ListCdf &c) {
+    c.S = softmax_exp_sum<8>(sc, n, m, lane);
+    if (long_uses_tiles(n, tiles)) c.total = cdf_total_tiles(sc, n, c.S, lane, tiles);
+    else c.total = cdf_total<8>(sc, n, c.S, lane, c.car);
+}
+static __device__ __noinline__ int cdf_draw_long(const float *sc, int n, const ListCdf &c, double u, int lane,
+                                                 const double *tiles) {
+    if (long_uses_tiles(n, tiles)) return cdf_pick_tiles(sc, n, c.S, c.total, u, lane, tiles);
+    return cdf_pick(sc, n, c.S, c.total, u, lane, c.car);
+}
+// (one draw: the same passes in one out-of-line call -- two calls here cost the per-walk kernels registers)
 static __device__ __noinline__ int choose_index_long(float *sc, int n, float m, double u, int lane, double *tiles) {
     float S;
     double car[2], total;
     if (tiles && ((n + 31) >> 5) <= SC_CAP / 2) {
-        // per-tile running totals in the (idle) shared score buffer: the draw finds its tile among hundreds directly
         S = softmax_exp_sum<8>(sc, n, m, lane);
         total = cdf_total_tiles(sc, n, S, lane, tiles);
         return cdf_pick_tiles(sc, n, S, total, u, lane, tiles);
@@ -274,16 +309,32 @@ static __device__ __noinline__ int choose_index_long(float *sc, int n, float m, 
     return cdf_pick(sc, n, S, total, u, lane, car);
 }
 
+// softmax + CDF over sc[0..n) given its max m (n >= 2); `tiles`: see cdf_prepare_long (lists longer than SC_CAP)
+__device__ __forceinline__ void cdf_prepare(float *sc, int n, float m, int lane, double *tiles, ListCdf &c) {
+    if (n <= 32) {
+        c.car[0] = tile1_cdf(sc, n, m, lane, c.total);
+    } else if (n > SC_CAP) {
+        cdf_prepare_long(sc, n, m, lane, tiles, c);
+    } else {
+        c.S = softmax_exp_sum(sc, n, m, lane);
+        c.total = cdf_total(sc, n, c.S, lane, c.car);
+    }
+}
+
+// the draw for uniform u from a prepared list.  All lanes return the index.
+__device__ __forceinline__ int cdf_draw(const float *sc, int n, const ListCdf &c, double u, int lane, const double *tiles) {
+    if (n <= 32) return tile1_pick(c.car[0], c.total, n, u, lane);
+    if (n > SC_CAP) return cdf_draw_long(sc, n, c, u, lane, tiles);
+    return cdf_pick(sc, n, c.S, c.total, u, lane, c.car);
+}
+
+// softmax + CDF + draw over sc[0..n) given its max m (== ggo_choose), n >= 2: a list drawn from once.  All lanes return
+// the index.
 __device__ __forceinline__ int choose_index(float *sc, int n, float m, double u, int lane, double *tiles = nullptr) {
     if (n <= 32) {
-        // one tile (the common case): S = 0 + T_0 = T_0, total = 0 + scan_31 = scan_31 and the carry of the draw is 0, so
-        // the canonical sequence collapses to ONE scan and ONE division per lane -- the same floats, bit for bit
-        const float e = (lane < n) ? exp_c(__fsub_rn(sc[lane], m)) : 0.0f;
-        const float S = warp_sum_butterfly(e);
-        const double x = warp_scan_ks((double)__fdiv_rn(e, S), lane);
-        const double total = __shfl_sync(FULL, x, 31);
-        const unsigned hit = __ballot_sync(FULL, (lane < n) && (__ddiv_rn(x, total) > u));
-        return hit ? __ffs(hit) - 1 : n - 1;
+        double total;
+        const double x = tile1_cdf(sc, n, m, lane, total);
+        return tile1_pick(x, total, n, u, lane);
     }
     if (n > SC_CAP) return choose_index_long(sc, n, m, u, lane, tiles);
     double car[2];

@@ -6,8 +6,10 @@ torch.profiler (CUDA activities only) for --passes passes and writes ONE JSON re
 
   levels[s]   device microseconds per pass of each kernel of level-synchronous step s (flat_dedupe / flat_enum /
               flat_choose / flat_draw and the table clear of a shared level), and the level's sizes read back from the
-              flat counters: records (walks that take step s), hub items (walks on a score-cached node) and distinct
-              keys (distinct (root slot, node) items of a shared level; 0 on a level that does not share);
+              flat counters: records (walks that take step s), hub items (walks on a score-cached node), distinct
+              keys (distinct (root slot, node) items of a shared level that are not score-cached; 0 on a level that
+              does not share) and hub owners / hub work items (distinct score-cached (root slot, node) groups of a
+              shared level and the work items they were split into; 0 where hub walks run per walk);
   stage       flat_start_kernel, the walk_kernel tail, and the whole walk stage (first to last of its kernels).
 
 The levels reuse kernel names, so a kernel is given to a level by launch order within the pass.  Load an A/B library
@@ -26,6 +28,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 FLAT_CTR_WORDS = 1 + 4 * 16          # csrc/walk.cu: FLAT_CTR_WORDS
+FLAT_CTR_ALL = FLAT_CTR_WORDS + 3 * 16   # csrc/walk.cu: FLAT_CTR_ALL (the hub group words follow the level words)
 
 
 def short_name(name):
@@ -135,7 +138,7 @@ def main():
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for s in range(args.passes):
             one_pass(2000 + s)
-            ctrs.append(plan._flat[:4 * FLAT_CTR_WORDS].clone())        # device copy, read after the region
+            ctrs.append(plan._flat[:4 * FLAT_CTR_ALL].clone())        # device copy, read after the region
         torch.cuda.synchronize()
     passes = split_levels(kernel_events(prof), args.passes)
     ctr = np.stack([c.view(torch.int32).cpu().numpy().astype(np.int64) for c in ctrs])   # [passes, words]
@@ -148,6 +151,8 @@ def main():
             "total_us": round(float(np.mean([sum(per.get(s, {}).values()) for per, _ in passes])) / 1e3, 2),
             "records": int(ctr[:, 1 + 4 * s].mean()), "hub_items": int(ctr[:, 1 + 4 * s + 1].mean()),
             "distinct_keys": int(ctr[:, 1 + 4 * s + 2].mean()),
+            "hub_owners": int(ctr[:, FLAT_CTR_WORDS + 3 * s].mean()),
+            "hub_work_items": int(ctr[:, FLAT_CTR_WORDS + 3 * s + 1].mean()),
         }
     rec = {
         "tool": "tools/profile_walk_levels.py", "label": args.label, "lib": os.path.basename(os.environ.get("GG_LIB") or _cabi._build.LIB),

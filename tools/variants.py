@@ -20,6 +20,7 @@ VARIANTS = {
     "unr2": ["GG_UNR=2"],
     "share0": ["GG_SHARE_LEVELS=0"],              # no shared level: every level runs flat_enum + flat_choose per walk
     "share23": ["GG_SHARE_LEVELS=0xC"],           # levels 2 and 3 shared (default: level 2)
+    "hub0": ["GG_SHARE_HUB=0"],                   # shared levels run their hub walks per walk (default: one warp per hub group)
 }
 
 
