@@ -28,6 +28,20 @@ __global__ void __launch_bounds__(256, 4) adam_kernel(long long n_node, int ld, 
     adam_rows<false, 2>(n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, grad_rows, grad_bias, row_slot, lr_t, b1, b2, eps);
 }
 
+// ld = 512: a row is four segments, so a warp keeps four in flight -- the whole row.  The lane that clears the row's slot
+// then does so after every lane that reads the slot has read it (the __syncwarp in adam_rows); with two segments per warp
+// the other half of the row would belong to another warp, which could find the slot already cleared.  (Four segments in
+// flight need the registers of 2 CTAs per SM; at 4 the kernel spills.)
+__global__ void __launch_bounds__(256, 2) adam_wide_kernel(long long n_node, int ld, float *__restrict__ emb,
+                                                        float *__restrict__ m_emb, float *__restrict__ v_emb,
+                                                        float *__restrict__ bias, float *__restrict__ m_bias,
+                                                        float *__restrict__ v_bias, const float *__restrict__ grad_rows,
+                                                        const float *__restrict__ grad_bias, int *__restrict__ row_slot,
+                                                        float lr_t, float b1, float b2, float eps) {
+    adam_rows<false, ADAM_WIDE_UNR>(n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, grad_rows, grad_bias, row_slot, lr_t, b1,
+                                    b2, eps);
+}
+
 // ---------------------------------------------------------------- the same sweep with TMA bulk copies (sm_90+)
 // The sweep is a pure stream (24 * N * ld bytes per step), so it is fed by the copy engine instead of per-thread loads:
 // one elected thread issues cp.async.bulk (global -> shared, completion on an mbarrier) for a tile of E, m and v, all
@@ -284,7 +298,7 @@ extern "C" int gg_adam_apply(int64_t n_node, int32_t ld, float *emb, float *m_em
     if (gg::g_adam_path < 0) gg::g_adam_path = gg::adam_path_from_name(getenv("GG_ADAM_PATH"));
     const int use_tma = gg::g_adam_path;
     GG_REQUIRE(emb && m_emb && v_emb && bias && m_bias && v_bias && grad_rows && grad_bias && row_slot, "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     if (n_node == 0) return 0;
     if (use_tma) {
         const long long n_tiles = (n_node * (long long)ld + gg::ADAM_TILE - 1) / gg::ADAM_TILE;
@@ -320,6 +334,15 @@ extern "C" int gg_adam_apply(int64_t n_node, int32_t ld, float *emb, float *m_em
     }
     const int q = ld / 4;                                                       // float4 per row
     const long long nseg = q >= 32 ? n_node * (q / 32) : (n_node + 32 / q - 1) / (32 / q);   // 512-byte segments
+    if (ld == gg::LD_MAX) {                                                     // 8 warps x 4 segments (one row each)
+        long long blocks = (nseg + 4 * 8 - 1) / (4 * 8);
+        const long long cap = (long long)gg::sm_count() * 16;
+        if (blocks > cap) blocks = cap;
+        gg::adam_wide_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(n_node, ld, emb, m_emb, v_emb, bias, m_bias,
+                                                                                 v_bias, grad_rows, grad_bias, row_slot, lr_t,
+                                                                                 beta1, beta2, eps);
+        return gg::check_cuda(cudaGetLastError(), "adam kernel launch");
+    }
     long long blocks = (nseg + 2 * 8 - 1) / (2 * 8);                            // 8 warps x 2 segments in flight
     const long long cap = (long long)gg::sm_count() * 16;
     if (blocks > cap) blocks = cap;

@@ -281,7 +281,7 @@ extern "C" int gg_dp_step(void *comm, int32_t mode, int32_t n_pairs, const int32
         // then the merge kernel waits for all ranks' flags of this step
         GG_REQUIRE((int64_t)c->world * nf <= c->capacity, "exchange buffer too small for this cap / ld");
         GG_REQUIRE(mode == 0 || mode == 1, "mode must be 0 (discriminator) or 1 (generator)");
-        GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+        GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
         const unsigned step_id = ++c->step;
         const int B = hi - lo;
         const size_t smem_g = gg::pair_grad_smem_bytes(B > 0 ? B : 1);
@@ -384,7 +384,7 @@ extern "C" int gg_dp_step_ex(void *comm, int32_t mode, int32_t n_pairs, const in
                         "gg_comm_use_p2p(comm, 0))");
     GG_REQUIRE(n_pairs > 0 && n_pairs <= DP_MAX_PAIRS, "n_pairs must be in 1 .. 2^30 - 4096");
     GG_REQUIRE(mode == 0 || mode == 1, "mode must be 0 (discriminator) or 1 (generator)");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     GG_REQUIRE(node_id && node_neighbor_id && aux && local_buf && gathered_buf, "null pointer");
     GG_REQUIRE(cap >= 2 * (((int64_t)n_pairs + c->world - 1) / c->world), "cap too small: need 2 * ceil(n_pairs / world)");
     int lo, hi;

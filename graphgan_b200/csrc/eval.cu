@@ -117,7 +117,7 @@ extern "C" int gg_pair_dot_f64(int64_t n_pairs, const int32_t *node_id, const in
                                int32_t ld, double *out, void *stream) {
     if (n_pairs == 0) return 0;
     GG_REQUIRE(node_id && node_neighbor_id && emb && out, "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     long long blocks = (n_pairs + 31) / 32;
     const long long cap = (long long)gg::sm_count() * 16;
     if (blocks > cap) blocks = cap;

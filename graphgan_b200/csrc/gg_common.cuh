@@ -33,6 +33,14 @@ int launch_exclusive_scan_i64(long long *a, long long n, long long *total_out, c
 
 constexpr unsigned FULL = 0xffffffffu;
 
+// The row strides (floats per embedding row) the kernels are built for: 32, 64, 128, 256 and 512.  Every entry point that
+// takes `ld` checks it here, and sampler.pad_embedding picks the stride by the same rule.
+constexpr int LD_MAX = 512;
+__host__ __device__ constexpr bool ld_supported(int ld) {
+    return ld == 32 || ld == 64 || ld == 128 || ld == 256 || ld == LD_MAX;
+}
+#define GG_LD_MESSAGE "ld must be 32, 64, 128, 256 or 512 (row stride in floats)"
+
 // Philox4x32-10 (Salmon et al. SC'11); only the first two output words are needed.
 __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3,
                                               uint32_t k0, uint32_t k1, uint32_t &o0, uint32_t &o1) {

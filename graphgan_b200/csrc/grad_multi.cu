@@ -307,7 +307,8 @@ __global__ void __launch_bounds__(256) mc_short_sums_kernel(int E, int ld, const
     }
 }
 
-// ---- 5b: long slots, one CTA each (taken from the list in any order), thread c < ld sums column c, thread ld the bias
+// ---- 5b: long slots, one CTA each (taken from the list in any order), thread c < ld sums column c, thread ld the bias (at
+// ld = LONG_THREADS there is no such thread: mc_long_bias_kernel sums it)
 __device__ __forceinline__ void cp_async16(void *dst, const void *src) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
@@ -358,6 +359,47 @@ __global__ void __launch_bounds__(LONG_THREADS, 1) mc_long_sums_kernel(int ld, c
         }
         if (tid < ld) grad_rows[(size_t)u * ld + tid] = acc;
         else if (tid == ld) grad_bias[u] = acc;
+    }
+}
+
+// ---- 5c (ld >= LONG_THREADS only): the bias of the long slots, which mc_long_sums_kernel has no thread left for.  One
+// warp per slot: every lane loads one entry's bias term per group of 32 entries, LONG_BIAS_TILES groups at a time (the
+// next LONG_BIAS_TILES groups' loads in flight while these are added), and the warp adds them in entry order through
+// shuffles -- the same +0-started __fadd_rn chain that thread `ld` would run, at one dependent add per entry.
+constexpr int LONG_BIAS_TILES = 8;
+__global__ void __launch_bounds__(256) mc_long_bias_kernel(int ld, const int *__restrict__ off, const float *__restrict__ terms,
+                                                           float *__restrict__ grad_bias, const int *__restrict__ long_list,
+                                                           const int *__restrict__ counters) {
+    constexpr int U = LONG_BIAS_TILES;
+    const int lane = threadIdx.x & 31;
+    const int warp = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), nwarps = (int)((gridDim.x * blockDim.x) >> 5);
+    const int ts = term_stride(ld), n_long = counters[0];
+    for (int k = warp; k < n_long; k += nwarps) {
+        const int u = long_list[k], lo = off[u], n = off[u + 1] - lo;
+        const float *b = terms + (size_t)lo * ts + ld;
+        float acc = 0.0f, nxt[U];
+#pragma unroll
+        for (int q = 0; q < U; ++q) nxt[q] = (32 * q + lane < n) ? __ldg(b + (size_t)(32 * q + lane) * ts) : 0.0f;
+        for (int e0 = 0; e0 < n; e0 += 32 * U) {
+            float cur[U];
+#pragma unroll
+            for (int q = 0; q < U; ++q) {
+                cur[q] = nxt[q];
+                const int e = e0 + 32 * (U + q) + lane;
+                nxt[q] = (e < n) ? __ldg(b + (size_t)e * ts) : 0.0f;
+            }
+#pragma unroll
+            for (int q = 0; q < U; ++q) {
+                const int left = n - (e0 + 32 * q);        // warp-uniform
+                if (left >= 32) {
+#pragma unroll
+                    for (int t = 0; t < 32; ++t) acc = __fadd_rn(acc, __shfl_sync(FULL, cur[q], t));
+                } else {
+                    for (int t = 0; t < left; ++t) acc = __fadd_rn(acc, __shfl_sync(FULL, cur[q], t));
+                }
+            }
+        }
+        if (lane == 0) grad_bias[u] = acc;
     }
 }
 
@@ -512,7 +554,7 @@ __global__ void __launch_bounds__(256) mg_sums_kernel(int cap, int ld, const flo
 extern "C" int gg_pair_grad_scratch_bytes(int32_t n_pairs, int32_t ld, int64_t *bytes) {
     GG_REQUIRE(bytes, "null pointer");
     GG_REQUIRE(n_pairs > 0 && n_pairs <= gg::MAX_PAIRS, "n_pairs must be in 1 .. 2^30 - 4096");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     *bytes = (int64_t)gg::carve(nullptr, n_pairs, ld).bytes;
     return 0;
 }
@@ -529,7 +571,7 @@ extern "C" int gg_pair_grad_ex(int32_t mode, int32_t n_pairs, int32_t batch_tota
                             uniq_ids, grad_rows, grad_bias, row_slot, stream);
     GG_REQUIRE(node_id && node_neighbor_id && aux && emb && bias && n_unique && uniq_ids && grad_rows && grad_bias && row_slot,
                "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     const gg::Scratch need = gg::carve(nullptr, n_pairs, ld);
     GG_REQUIRE(scratch && scratch_bytes >= (int64_t)need.bytes, "scratch is null or smaller than gg_pair_grad_scratch_bytes");
     GG_REQUIRE(((uintptr_t)scratch & 255) == 0, "scratch must be 256-byte aligned");
@@ -558,6 +600,12 @@ extern "C" int gg_pair_grad_ex(int32_t mode, int32_t n_pairs, int32_t batch_tota
         gg::mc_long_sums_kernel<<<long_grid, gg::LONG_THREADS, smem, st>>>(ld, s.off, s.terms, grad_rows, grad_bias, s.long_list,
                                                                             s.counters);
         GG_CHECK(cudaGetLastError());
+        if (ld >= gg::LONG_THREADS) {
+            int bias_blocks = (E / (gg::SHORT_MAX + 1) + 7) / 8;     // a warp per possible long slot, 8 per CTA
+            if (bias_blocks > gg::sm_count() * 8) bias_blocks = gg::sm_count() * 8;
+            gg::mc_long_bias_kernel<<<bias_blocks, 256, 0, st>>>(ld, s.off, s.terms, grad_bias, s.long_list, s.counters);
+            GG_CHECK(cudaGetLastError());
+        }
     }
     return 0;
 }
@@ -566,7 +614,7 @@ extern "C" int gg_grad_merge_scratch_bytes(int32_t world, int32_t cap, int32_t l
     GG_REQUIRE(bytes, "null pointer");
     GG_REQUIRE(world >= 1 && cap >= 1, "world and cap must be >= 1");
     GG_REQUIRE((int64_t)world * cap <= 2 * gg::MAX_PAIRS, "world * cap must be at most 2^31 - 8192 entries");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     *bytes = (int64_t)gg::carve_merge(nullptr, (long long)world * cap).bytes;
     return 0;
 }
@@ -580,7 +628,7 @@ extern "C" int gg_grad_merge_ex(int32_t world, int32_t cap, int32_t ld, const fl
     if ((int64_t)world * cap <= 2 * GG_MAX_BATCH * 8 && !(flags & GG_GRAD_MULTI_CTA))
         return gg_grad_merge(world, cap, ld, gathered, n_unique, uniq_ids, grad_rows, grad_bias, row_slot, stream);
     GG_REQUIRE(gathered && n_unique && uniq_ids && grad_rows && grad_bias && row_slot, "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     GG_REQUIRE(world == 1 || cap % 2 == 0, "cap must be even when world > 1 (16-byte aligned blocks)");
     GG_REQUIRE(((uintptr_t)gathered & 15) == 0, "gathered must be 16-byte aligned");
     const int E = world * cap;

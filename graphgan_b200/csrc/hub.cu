@@ -17,6 +17,12 @@
 namespace gg {
 namespace {
 
+// ld = 512: the warp's current row in dynamic shared memory (WIDE_ROW_BYTES per warp; walk_common.cuh)
+__device__ __forceinline__ float *hub_wide_row() {
+    extern __shared__ __align__(16) unsigned char hub_smem[];
+    return reinterpret_cast<float *>(hub_smem + (size_t)(threadIdx.x >> 5) * WIDE_ROW_BYTES);
+}
+
 template <int CPL>
 __global__ void __launch_bounds__(WARPS_PER_CTA * 32)
 hub_score_kernel(long long n_tiles, const int *__restrict__ tile_node, const long long *__restrict__ tile_begin,
@@ -29,9 +35,15 @@ hub_score_kernel(long long n_tiles, const int *__restrict__ tile_node, const lon
         const int u = tile_node[t];
         const long long e0 = tile_begin[t], a1 = indptr[u + 1];
         const int n = (int)((a1 - e0) < tile_edges ? (a1 - e0) : tile_edges);
-        float4 c4[CPL];
-        load_row<CPL>(emb, ld, u, lane & 7, c4);
-        score_edges<CPL>(emb, bias, ld, c4, adj, e0, n, edge_score + e0, u, lane);
+        if constexpr (CPL == WIDE_CPL) {
+            float *s_row = hub_wide_row();
+            load_row_wide(emb, ld, u, s_row, lane);
+            score_edges_wide(emb, bias, ld, s_row, adj, e0, n, edge_score + e0, u, lane);
+        } else {
+            float4 c4[CPL];
+            load_row<CPL>(emb, ld, u, lane & 7, c4);
+            score_edges<CPL>(emb, bias, ld, c4, adj, e0, n, edge_score + e0, u, lane);
+        }
     }
 }
 
@@ -51,13 +63,22 @@ root_cdf_kernel(const __grid_constant__ gg_walk_desc d, float *__restrict__ root
             for (int i = lane; i < n; i += 32) sc[i] = __ldg(d.edge_score + a0 + i);
             __syncwarp();
         } else {
-            float4 c4[CPL];
-            load_row<CPL>(d.emb, d.ld, root, lane & 7, c4);
-            score_edges<CPL>(d.emb, d.bias, d.ld, c4, d.adj, a0, n, sc, root, lane);
+            if constexpr (CPL == WIDE_CPL) {
+                float *s_row = hub_wide_row();
+                load_row_wide(d.emb, d.ld, root, s_row, lane);
+                score_edges_wide(d.emb, d.bias, d.ld, s_row, d.adj, a0, n, sc, root, lane);
+            } else {
+                float4 c4[CPL];
+                load_row<CPL>(d.emb, d.ld, root, lane & 7, c4);
+                score_edges<CPL>(d.emb, d.bias, d.ld, c4, d.adj, a0, n, sc, root, lane);
+            }
         }
         cdf_store(sc, n, root_q + o, lane);
     }
 }
+
+// dynamic shared memory of a launch (only ld = 512 keeps the current row there)
+constexpr int hub_smem_bytes(int cpl) { return cpl == WIDE_CPL ? WARPS_PER_CTA * WIDE_ROW_BYTES : 0; }
 
 }  // namespace
 }  // namespace gg
@@ -67,13 +88,14 @@ extern "C" int gg_hub_scores(int64_t n_tiles, const int32_t *tile_node, const in
                              float *edge_score, void *stream) {
     if (n_tiles == 0) return 0;
     GG_REQUIRE(tile_node && tile_begin && indptr && adj && emb && bias && edge_score, "null pointer");
-    GG_REQUIRE(tile_edges > 0 && ld > 0 && ld % 32 == 0, "bad tile_edges / ld");
+    GG_REQUIRE(tile_edges > 0, "bad tile_edges");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     long long blocks = (n_tiles + gg::WARPS_PER_CTA - 1) / gg::WARPS_PER_CTA;
     const long long cap = (long long)gg::sm_count() * 8;
     if (blocks > cap) blocks = cap;
     cudaStream_t st = (cudaStream_t)stream;
 #define GG_LAUNCH(C)                                                                                           \
-    gg::hub_score_kernel<C><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, 0, st>>>(                              \
+    gg::hub_score_kernel<C><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, gg::hub_smem_bytes(C), st>>>(          \
         n_tiles, tile_node, (const long long *)tile_begin, tile_edges, (const long long *)indptr, adj, emb, bias, ld, \
         edge_score)
     switch (ld / 32) {
@@ -81,7 +103,8 @@ extern "C" int gg_hub_scores(int64_t n_tiles, const int32_t *tile_node, const in
         case 2: GG_LAUNCH(2); break;
         case 4: GG_LAUNCH(4); break;
         case 8: GG_LAUNCH(8); break;
-        default: gg::set_error("gg_hub_scores: unsupported ld %d (supported: 32, 64, 128, 256)", ld); return 2;
+        case 16: GG_LAUNCH(16); break;
+        default: gg::set_error("gg_hub_scores: unsupported ld %d (supported: 32, 64, 128, 256, 512)", ld); return 2;
     }
 #undef GG_LAUNCH
     return gg::check_cuda(cudaGetLastError(), "hub score kernel launch");
@@ -93,7 +116,7 @@ extern "C" int gg_root_cdf(const gg_walk_desc *dp, float *root_sc, double *root_
     GG_REQUIRE(root_sc && root_q, "null pointer");
     const gg_walk_desc &d = *dp;
     GG_REQUIRE(d.roots && d.indptr && d.adj && d.emb && d.bias && d.rq_ptr, "null pointer in descriptor");
-    GG_REQUIRE(d.ld > 0 && d.ld % 32 == 0, "ld must be a positive multiple of 32");
+    GG_REQUIRE(gg::ld_supported(d.ld), GG_LD_MESSAGE);
     if (d.n_roots == 0) return 0;
     long long blocks = (d.n_roots + gg::WARPS_PER_CTA - 1) / gg::WARPS_PER_CTA;
     const long long cap = (long long)gg::sm_count() * 8;
@@ -104,7 +127,10 @@ extern "C" int gg_root_cdf(const gg_walk_desc *dp, float *root_sc, double *root_
         case 2: gg::root_cdf_kernel<2><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, 0, st>>>(d, root_sc, root_q); break;
         case 4: gg::root_cdf_kernel<4><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, 0, st>>>(d, root_sc, root_q); break;
         case 8: gg::root_cdf_kernel<8><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, 0, st>>>(d, root_sc, root_q); break;
-        default: gg::set_error("gg_root_cdf: unsupported ld %d (supported: 32, 64, 128, 256)", d.ld); return 2;
+        case 16:
+            gg::root_cdf_kernel<16><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, gg::hub_smem_bytes(16), st>>>(d, root_sc, root_q);
+            break;
+        default: gg::set_error("gg_root_cdf: unsupported ld %d (supported: 32, 64, 128, 256, 512)", d.ld); return 2;
     }
     return gg::check_cuda(cudaGetLastError(), "root cdf kernel launch");
 }

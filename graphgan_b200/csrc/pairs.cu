@@ -130,7 +130,7 @@ extern "C" int gg_pair_reward(int64_t n_pairs, const int32_t *node_id, const int
                               const float *bias, int32_t ld, float *reward, void *stream) {
     if (n_pairs == 0) return 0;
     GG_REQUIRE(node_id && node_neighbor_id && emb && bias && reward, "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     long long blocks = (n_pairs + 31) / 32;  // 8 warps x 4 pairs per pass
     const long long cap = (long long)gg::sm_count() * 8;
     if (blocks > cap) blocks = cap;
@@ -142,7 +142,7 @@ extern "C" int gg_pair_reward(int64_t n_pairs, const int32_t *node_id, const int
 extern "C" int gg_all_score(int64_t n_node, const float *emb, const float *bias, int32_t ld, float *out, void *stream) {
     if (n_node == 0) return 0;
     GG_REQUIRE(emb && bias && out, "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     GG_REQUIRE(n_node <= 46340, "all_score is only materialised for small graphs (N*N must fit int32 range of tests)");
     gg::all_score_kernel<<<gg::sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n_node, emb, bias, ld, out);
     return gg::check_cuda(cudaGetLastError(), "all_score kernel launch");
@@ -156,7 +156,7 @@ extern "C" int gg_pair_grad(int32_t mode, int32_t n_pairs, int32_t batch_total, 
     GG_REQUIRE(n_pairs > 0 && n_pairs <= GG_MAX_BATCH, "batch size out of range");
     GG_REQUIRE(node_id && node_neighbor_id && aux && emb && bias && n_unique && uniq_ids && grad_rows && grad_bias && row_slot,
                "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     const size_t smem = gg::pair_grad_smem_bytes(n_pairs);
     gg::pair_grad_kernel<<<1, gg::GRAD_THREADS, smem, (cudaStream_t)stream>>>(
         mode, n_pairs, batch_total > 0 ? batch_total : n_pairs, node_id, node_neighbor_id, aux, emb, bias, ld, lambda,
@@ -170,7 +170,7 @@ extern "C" int gg_grad_merge(int32_t world, int32_t cap, int32_t ld, const float
                              int32_t *uniq_ids, float *grad_rows, float *grad_bias, int32_t *row_slot, void *stream) {
     GG_REQUIRE(world > 0 && cap > 0 && (int64_t)world * cap <= 2 * GG_MAX_BATCH * 8, "too many entries to merge");
     GG_REQUIRE(gathered && n_unique && uniq_ids && grad_rows && grad_bias && row_slot, "null pointer");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     const size_t smem = (size_t)world * cap * 2 * 4;
     GG_REQUIRE(smem <= 200 * 1024, "merge exceeds shared memory");
     if (smem > 48 * 1024)

@@ -92,8 +92,9 @@ __device__ __forceinline__ void add_release(unsigned long long *p, unsigned long
     asm volatile("red.release.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
-template <int NT>
-__global__ void __launch_bounds__(NT, 1) train_loop_kernel(const __grid_constant__ LoopArgs a) {
+// SWEEP_UNR: segments per warp of the sweep (adam_rows); ld = 512 needs ADAM_WIDE_UNR (the warp clears the rows' slots)
+template <int NT, int SWEEP_UNR>
+__device__ __forceinline__ void train_loop_body(const LoopArgs &a) {
     extern __shared__ int smem[];
     unsigned long long *ready = a.sync_words, *done = a.sync_words + 1;
     float b1p = a.beta1_power, b2p = a.beta2_power;
@@ -116,7 +117,7 @@ __global__ void __launch_bounds__(NT, 1) train_loop_kernel(const __grid_constant
         const long long t1 = clk ? clock64() : 0;
         // lr_t = lr * sqrt(1 - beta2^t) / (1 - beta1^t): the same fp32 operation sequence as the host loop
         const float lr_t = __fdiv_rn(__fmul_rn(a.lr, __fsqrt_rn(__fsub_rn(1.0f, b2p))), __fsub_rn(1.0f, b1p));
-        adam_rows<true, 2, false>(a.n_node, a.ld, a.emb, a.m_emb, a.v_emb, a.bias, a.m_bias, a.v_bias, a.grad_rows, a.grad_bias,
+        adam_rows<true, SWEEP_UNR, false>(a.n_node, a.ld, a.emb, a.m_emb, a.v_emb, a.bias, a.m_bias, a.v_bias, a.grad_rows, a.grad_bias,
                                   a.row_slot, lr_t, a.beta1, a.beta2, a.eps);
         b1p = __fmul_rn(b1p, a.beta1);
         b2p = __fmul_rn(b2p, a.beta2);
@@ -133,6 +134,12 @@ __global__ void __launch_bounds__(NT, 1) train_loop_kernel(const __grid_constant
         a.sync_words[2] = (unsigned long long)c_grad; a.sync_words[3] = (unsigned long long)c_sweep;
         a.sync_words[4] = (unsigned long long)c_wait; a.sync_words[5] = (unsigned long long)a.n_starts;
     }
+}
+template <int NT>
+__global__ void __launch_bounds__(NT, 1) train_loop_kernel(const __grid_constant__ LoopArgs a) { train_loop_body<NT, 2>(a); }
+template <int NT>
+__global__ void __launch_bounds__(NT, 1) train_loop_wide_kernel(const __grid_constant__ LoopArgs a) {
+    train_loop_body<NT, ADAM_WIDE_UNR>(a);
 }
 
 // ---------------------------------------------------------------- fused step loop
@@ -289,7 +296,7 @@ extern "C" int gg_train_loop(int32_t mode, int64_t n_rows, const int64_t *start_
     GG_REQUIRE(start_list_dev && beta1_power && beta2_power && sync_words, "null pointer");
     GG_REQUIRE(batch_size > 0 && batch_size <= GG_MAX_BATCH, "batch size out of range");
     GG_REQUIRE(mode == 0 || mode == 1, "mode must be 0 (discriminator) or 1 (generator)");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256 (row stride in floats)");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     if (n_starts == 0) return 0;
     int dev = 0, coop = 0, per_sm = 0;
     GG_CHECK(cudaGetDevice(&dev));
@@ -298,8 +305,9 @@ extern "C" int gg_train_loop(int32_t mode, int64_t n_rows, const int64_t *start_
     const size_t smem = gg::pair_grad_smem_bytes(batch_size);
     // 512 threads: the 64-register ceiling of a 1024-thread CTA makes the fused body spill (measured 18.7 vs 13.5 us/step)
     constexpr int NT = 512;
-    const void *kern = (const void *)gg::train_loop_kernel<NT>;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gg::train_loop_kernel<NT>, NT, smem));
+    const bool wide = ld == gg::LD_MAX;
+    const void *kern = wide ? (const void *)gg::train_loop_wide_kernel<NT> : (const void *)gg::train_loop_kernel<NT>;
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, NT, smem));
     GG_REQUIRE(per_sm >= 1, "step loop kernel does not fit on an SM");
     // one sweep iteration per warp (2 segments of 512 B in flight), at most one CTA per SM
     long long ctas = (n_node + 63) / 64;
@@ -334,7 +342,7 @@ extern "C" int gg_train_fused(int32_t mode, int64_t n_rows, const int64_t *start
     GG_REQUIRE(emb && m_emb && v_emb && bias && m_bias && v_bias && node_id && node_neighbor_id && aux, "null pointer");
     GG_REQUIRE(batch_size > 0 && batch_size <= GG_MAX_BATCH, "batch size out of range");
     GG_REQUIRE(mode == 0 || mode == 1, "mode must be 0 (discriminator) or 1 (generator)");
-    GG_REQUIRE(ld == 32 || ld == 64 || ld == 128 || ld == 256, "ld must be 32, 64, 128 or 256");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
     if (n_starts == 0) return 0;
     constexpr int NT = 512, UNR = 2, W = NT / 32;
     int dev = 0, coop = 0, per_sm = 0;

@@ -266,6 +266,8 @@ __device__ __forceinline__ void pair_grad_body(int *smem, int mode, int B, int b
 // loads of all of them are issued before the first use; only the rare rows with a gradient add a dependent load.
 // The lane owning a row's first columns also updates the row's bias and clears its slot (after the warp has read
 // it; PRE = its bias loads are issued with the others, which costs registers).  COH: the gradient slots were written earlier in the same kernel by another SM -> read them through L2.
+// At ld = 512 (four segments per row) UNR must be a multiple of 4 (ADAM_WIDE_UNR): the whole row in one warp.
+constexpr int ADAM_WIDE_UNR = 4;
 template <bool COH, int UNR, bool PRE = true>
 __device__ __forceinline__ void adam_rows(long long n_node, int ld, float *emb, float *m_emb, float *v_emb, float *bias,
                                           float *m_bias, float *v_bias, const float *grad_rows, const float *grad_bias,

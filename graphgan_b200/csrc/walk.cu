@@ -177,9 +177,15 @@ __device__ __forceinline__ void build_list(const gg_walk_desc &d, const uint32_t
     // whatever the score is, so neither the score nor the CDF is computed (leaves of the BFS tree: [father])
     if (n <= 1) return;
     if (!cached || inc_father) {
-        float4 c4[CPL];
-        load_row<CPL>(d.emb, d.ld, cur, lane & 7, c4);
-        score_list<CPL>(d.emb, d.bias, d.ld, c4, ids, sc, cached ? 1 : n, cur, lane);
+        if constexpr (CPL == WIDE_CPL) {
+            float *s_row = walk_wide_row(s_sc);
+            load_row_wide(d.emb, d.ld, cur, s_row, lane);
+            score_list_wide(d.emb, d.bias, d.ld, s_row, ids, sc, cached ? 1 : n, cur, lane);
+        } else {
+            float4 c4[CPL];
+            load_row<CPL>(d.emb, d.ld, cur, lane & 7, c4);
+            score_list<CPL>(d.emb, d.bias, d.ld, c4, ids, sc, cached ? 1 : n, cur, lane);
+        }
         rows_gathered += 1u + (unsigned)(cached ? 1 : n);
     }
     if (cached) {
@@ -340,7 +346,7 @@ __global__ void root_step_kernel(const __grid_constant__ gg_walk_desc d) {
 constexpr int S1_SINGLES = GG_S1_SINGLES, S1_CHUNK = 16;
 
 template <int CPL>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) step1_cdf_kernel(const __grid_constant__ gg_walk_desc d) {
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, walk_min_ctas(CPL)) step1_cdf_kernel(const __grid_constant__ gg_walk_desc d) {
     extern __shared__ __align__(16) unsigned char walk_smem[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     float *s_sc = reinterpret_cast<float *>(walk_smem + (size_t)wid * WALK_SMEM_PER_WARP);
@@ -468,7 +474,7 @@ constexpr int HUB_GROUP_MAX = GG_HUB_GROUP_MAX;
 static_assert(HUB_GROUP_MAX > 0 && HUB_GROUP_MAX % 32 == 0, "hub work items are whole warps of walks");
 
 template <int CPL>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) walk_kernel(const __grid_constant__ gg_walk_desc d,
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, walk_min_ctas(CPL)) walk_kernel(const __grid_constant__ gg_walk_desc d,
                                                                                  const FlatView fv, const int tail_mode) {
     extern __shared__ __align__(16) unsigned char walk_smem[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -892,7 +898,7 @@ __global__ void __launch_bounds__(FLAT_ENUM_WARPS * 32, 6) flat_enum_kernel(cons
 // SHARED: the items that are not score-cached are the level's distinct keys (fv.uniq); their CDF is stored for
 // flat_draw_kernel instead of being drawn from.  Hub items are the same either way.
 template <int CPL, bool SHARED>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose_kernel(const __grid_constant__ gg_walk_desc d,
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, walk_min_ctas(CPL)) flat_choose_kernel(const __grid_constant__ gg_walk_desc d,
                                                                                         const FlatView fv, const int s) {
     extern __shared__ __align__(16) unsigned char walk_smem[];
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -1016,11 +1022,14 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, WALK_MIN_CTAS) flat_choose
                 n = nrec & 0x3fffffff;
                 inc_father = (nrec >> 30) & 1;
                 const int *ids = fv.pool_ids + (size_t)i * (size_t)fv.stride;
-                float4 c4[CPL];
-                load_row<CPL>(d.emb, d.ld, cur, lane & 7, c4);
+                float4 c4[CPL];                                          // (ld = 512: the row goes to shared memory)
+                float *s_row = CPL == WIDE_CPL ? walk_wide_row(s_sc) : nullptr;
+                if constexpr (CPL == WIDE_CPL) load_row_wide(d.emb, d.ld, cur, s_row, lane);
+                else load_row<CPL>(d.emb, d.ld, cur, lane & 7, c4);
                 const int root = d.roots[slot];
                 const uint32_t k = (uint32_t)(w - __ldg(d.walk_ptr + slot));
-                score_list<CPL>(d.emb, d.bias, d.ld, c4, ids, s_sc, n, cur, lane);
+                if constexpr (CPL == WIDE_CPL) score_list_wide(d.emb, d.bias, d.ld, s_row, ids, s_sc, n, cur, lane);
+                else score_list<CPL>(d.emb, d.bias, d.ld, c4, ids, s_sc, n, cur, lane);
                 rows_gathered += 1u + (unsigned)n;
                 const float m = list_max(s_sc, n, lane);
                 if (SHARED) {
@@ -1096,9 +1105,10 @@ size_t flat_layout(void *buf, long long n_walks, int hub_threshold, int steps, F
 
 // ---------------------------------------------------------------- reference-order (stream) kernel
 // One warp replays the reference's sequential consumption of a uniform stream: a draw per
-// root (graph_gan.py:189/209), a draw per choice (:262), stop at a root's first void.
+// root (graph_gan.py:189/209), a draw per choice (:262), stop at a root's first void.  (ld = 512: one CTA per SM is
+// declared so that ptxas gives the kernel the registers of the streamed candidate row instead of spilling it.)
 template <int CPL>
-__global__ void __launch_bounds__(32) walk_stream_kernel(const __grid_constant__ gg_walk_desc d) {
+__global__ void __launch_bounds__(32, CPL == WIDE_CPL ? 1 : 0) walk_stream_kernel(const __grid_constant__ gg_walk_desc d) {
     extern __shared__ __align__(16) unsigned char walk_smem[];
     float *s_sc = reinterpret_cast<float *>(walk_smem);
     int *s_ids = reinterpret_cast<int *>(s_sc + SC_CAP);
@@ -1242,6 +1252,9 @@ __global__ void emit_rows_kernel(long long n_roots, const int *__restrict__ root
 }
 
 int grid_ctas() { return sm_count() * WALK_MIN_CTAS; }
+// CTAs of a walk kernel launch (ld = 512: fewer per SM, so never more than grid_ctas(), which sizes the scratch)
+int walk_ctas(int cpl) { return sm_count() * walk_min_ctas(cpl); }
+static_assert(WIDE_MIN_CTAS <= WALK_MIN_CTAS, "the walk scratch is sized for grid_ctas() warps");
 
 }  // namespace
 }  // namespace gg
@@ -1262,7 +1275,7 @@ extern "C" int gg_walk_flat_bytes(int64_t n_walks, int32_t hub_threshold, int32_
 extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
     GG_REQUIRE(dp, "null descriptor");
     const gg_walk_desc &d = *dp;
-    GG_REQUIRE(d.ld > 0 && d.ld % 32 == 0, "ld must be a positive multiple of 32");
+    GG_REQUIRE(gg::ld_supported(d.ld), GG_LD_MESSAGE);
     if (d.n_walks == 0 || d.n_roots == 0) return 0;   // nothing to do (empty batches carry null pointers)
     GG_REQUIRE(d.emb && d.bias && d.indptr && d.adj && d.roots && d.tree_bits && d.walk_ptr, "null graph/embedding pointer");
     GG_REQUIRE(d.tree_words > 0, "tree_words missing (gg_tree_words)");
@@ -1295,14 +1308,15 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
         switch (cpl) {
 #define GG_STREAM(C)                                                                                                  \
     GG_CHECK(cudaFuncSetAttribute(gg::walk_stream_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,            \
-                                  gg::WALK_SMEM_PER_WARP));                                                          \
-    gg::walk_stream_kernel<C><<<1, 32, gg::WALK_SMEM_PER_WARP, st>>>(d)
+                                  gg::walk_smem_bytes(C, 1)));                                                       \
+    gg::walk_stream_kernel<C><<<1, 32, gg::walk_smem_bytes(C, 1), st>>>(d)
             case 1: GG_STREAM(1); break;
             case 2: GG_STREAM(2); break;
             case 4: GG_STREAM(4); break;
             case 8: GG_STREAM(8); break;
+            case 16: GG_STREAM(16); break;
 #undef GG_STREAM
-            default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256)", d.ld); return 2;
+            default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256, 512)", d.ld); return 2;
         }
     } else {
         const int ctas = gg::grid_ctas();
@@ -1316,14 +1330,15 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
             GG_CHECK(cudaGetLastError());
 #define GG_S1(C)                                                                                                      \
     GG_CHECK(cudaFuncSetAttribute(gg::step1_cdf_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,              \
-                                  gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP));                                      \
-    gg::step1_cdf_kernel<C><<<ctas, gg::WARPS_PER_CTA * 32, gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP, st>>>(d)
+                                  gg::walk_smem_bytes(C, gg::WARPS_PER_CTA)));                                      \
+    gg::step1_cdf_kernel<C><<<gg::walk_ctas(C), gg::WARPS_PER_CTA * 32, gg::walk_smem_bytes(C, gg::WARPS_PER_CTA), st>>>(d)
             switch (cpl) {
                 case 1: GG_S1(1); break;
                 case 2: GG_S1(2); break;
                 case 4: GG_S1(4); break;
                 case 8: GG_S1(8); break;
-                default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256)", d.ld); return 2;
+            case 16: GG_S1(16); break;
+                default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256, 512)", d.ld); return 2;
             }
 #undef GG_S1
             GG_CHECK(cudaGetLastError());
@@ -1368,19 +1383,20 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
 #define GG_FLAT(C)                                                                                                    \
     if (shared) {                                                                                                    \
         GG_CHECK(cudaFuncSetAttribute(gg::flat_choose_kernel<C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                      gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP));                                  \
-        gg::flat_choose_kernel<C, true><<<ctas, gg::WARPS_PER_CTA * 32, gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP, st>>>(d, fv, s); \
+                                      gg::walk_smem_bytes(C, gg::WARPS_PER_CTA)));                                  \
+        gg::flat_choose_kernel<C, true><<<gg::walk_ctas(C), gg::WARPS_PER_CTA * 32, gg::walk_smem_bytes(C, gg::WARPS_PER_CTA), st>>>(d, fv, s); \
     } else {                                                                                                         \
         GG_CHECK(cudaFuncSetAttribute(gg::flat_choose_kernel<C, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                      gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP));                                  \
-        gg::flat_choose_kernel<C, false><<<ctas, gg::WARPS_PER_CTA * 32, gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP, st>>>(d, fv, s); \
+                                      gg::walk_smem_bytes(C, gg::WARPS_PER_CTA)));                                  \
+        gg::flat_choose_kernel<C, false><<<gg::walk_ctas(C), gg::WARPS_PER_CTA * 32, gg::walk_smem_bytes(C, gg::WARPS_PER_CTA), st>>>(d, fv, s); \
     }
                     case 1: GG_FLAT(1); break;
                     case 2: GG_FLAT(2); break;
                     case 4: GG_FLAT(4); break;
                     case 8: GG_FLAT(8); break;
+            case 16: GG_FLAT(16); break;
 #undef GG_FLAT
-                    default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256)", d.ld); return 2;
+                    default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256, 512)", d.ld); return 2;
                 }
                 GG_CHECK(cudaGetLastError());
                 if (shared) {
@@ -1393,14 +1409,15 @@ extern "C" int gg_walk_sample(const gg_walk_desc *dp, void *stream) {
         switch (cpl) {
 #define GG_WALK(C)                                                                                                    \
     GG_CHECK(cudaFuncSetAttribute(gg::walk_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,                   \
-                                  gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP));                                      \
-    gg::walk_kernel<C><<<ctas, gg::WARPS_PER_CTA * 32, gg::WARPS_PER_CTA * gg::WALK_SMEM_PER_WARP, st>>>(d, fv, tail_mode)
+                                  gg::walk_smem_bytes(C, gg::WARPS_PER_CTA)));                                      \
+    gg::walk_kernel<C><<<gg::walk_ctas(C), gg::WARPS_PER_CTA * 32, gg::walk_smem_bytes(C, gg::WARPS_PER_CTA), st>>>(d, fv, tail_mode)
             case 1: GG_WALK(1); break;
             case 2: GG_WALK(2); break;
             case 4: GG_WALK(4); break;
             case 8: GG_WALK(8); break;
+            case 16: GG_WALK(16); break;
 #undef GG_WALK
-            default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256)", d.ld); return 2;
+            default: gg::set_error("gg_walk_sample: unsupported ld %d (supported: 32, 64, 128, 256, 512)", d.ld); return 2;
         }
     }
     return gg::check_cuda(cudaGetLastError(), "walk kernel launch");

@@ -126,6 +126,83 @@ __device__ __forceinline__ void score_edges(const float *__restrict__ emb, const
     __syncwarp();
 }
 
+// ---- ld = 512 (CPL = 16).  The current row (16 float4 per lane) and two candidate rows (32 more) do not fit in registers,
+// so the warp keeps the current row in shared memory (WIDE_ROW_BYTES, one copy for the four groups) and each group streams
+// ONE candidate row per iteration: 16 float4 per lane in flight, as many bytes per round trip as the two half-as-wide rows
+// of CPL = 8.  Lane g still owns chunks g, g + 8, ..., g + 120 and runs one fma chain over them in that order, so a score
+// is the same bits as the register path's.  The walk kernels append the rows after their per-warp blocks and run at
+// WIDE_MIN_CTAS CTAs per SM (3 x (8 x 9 488 + 16 KB) does not fit in the SM's 228 KB; 2 x 92 KB does).
+constexpr int WIDE_CPL = 16;
+constexpr int WIDE_ROW_BYTES = WIDE_CPL * 32 * 4;
+constexpr int WIDE_MIN_CTAS = 2;
+__host__ __device__ constexpr int walk_min_ctas(int cpl) { return cpl == WIDE_CPL ? WIDE_MIN_CTAS : WALK_MIN_CTAS; }
+// dynamic shared memory of a walk kernel of `nwarps` warps
+__host__ __device__ constexpr int walk_smem_bytes(int cpl, int nwarps) {
+    return nwarps * (WALK_SMEM_PER_WARP + (cpl == WIDE_CPL ? WIDE_ROW_BYTES : 0));
+}
+static_assert(WALK_SMEM_PER_WARP % 16 == 0 && WIDE_ROW_BYTES % 16 == 0, "the row buffers are read as float4");
+static_assert(WIDE_MIN_CTAS * walk_smem_bytes(WIDE_CPL, WARPS_PER_CTA) <= 227 * 1024, "ld = 512 walk CTAs must fit on an SM");
+
+// the warp's row buffer of a walk kernel: s_sc is the warp's block of the per-warp layout (blockDim.x / 32 blocks)
+__device__ __forceinline__ float *walk_wide_row(float *s_sc) {
+    const int nw = blockDim.x >> 5, wid = threadIdx.x >> 5;
+    return reinterpret_cast<float *>(reinterpret_cast<unsigned char *>(s_sc) + (size_t)(nw - wid) * WALK_SMEM_PER_WARP +
+                                     (size_t)wid * WIDE_ROW_BYTES);
+}
+
+// the row of `node` into the warp's row buffer (the previous list's scoring has finished: score_* end with __syncwarp)
+__device__ __forceinline__ void load_row_wide(const float *__restrict__ emb, int ld, int node, float *s_row, int lane) {
+    const float *crow = emb + (size_t)node * (size_t)ld;
+#pragma unroll
+    for (int k = 0; k < WIDE_CPL / 4; ++k)
+        *reinterpret_cast<float4 *>(s_row + 4 * (lane + 32 * k)) = ldg4(crow + 4 * (lane + 32 * k));
+    __syncwarp();
+}
+
+// score of the candidate row `r` (this lane's chunks) against the row in s_row: the canonical dot, group-reduced
+__device__ __forceinline__ float wide_dot(const float *s_row, const float *r, int g) {
+    float4 x[WIDE_CPL];
+#pragma unroll
+    for (int c = 0; c < WIDE_CPL; ++c) x[c] = ldg4(r + 32 * c);
+    float s = 0.0f;
+#pragma unroll
+    for (int c = 0; c < WIDE_CPL; ++c) s = fma4(*reinterpret_cast<const float4 *>(s_row + 4 * g + 32 * c), x[c], s);
+    return group8_sum(s);
+}
+
+// score_list for ld = 512: one candidate per group per iteration
+__device__ __forceinline__ void score_list_wide(const float *__restrict__ emb, const float *__restrict__ bias, int ld,
+                                                const float *s_row, const int *ids, float *sc, int n, int fallback, int lane) {
+    const int grp = lane >> 3, g = lane & 7;
+    int c_n = (grp < n) ? ids[grp] : fallback;
+    for (int i0 = 0; i0 < n; i0 += 4) {
+        const int i = i0 + grp;
+        const int c = c_n;
+        c_n = (i + 4 < n) ? ids[i + 4] : fallback;   // (the next id in flight behind this row, see score_list)
+        const float b = __ldg(bias + c);
+        const float s = wide_dot(s_row, emb + (size_t)c * (size_t)ld + 4 * g, g);
+        if (g == 0 && i < n) sc[i] = __fadd_rn(s, b);
+    }
+    __syncwarp();
+}
+
+// score_edges for ld = 512
+__device__ __forceinline__ void score_edges_wide(const float *__restrict__ emb, const float *__restrict__ bias, int ld,
+                                                 const float *s_row, const int *__restrict__ adj, long long e0, int n,
+                                                 float *out, int fallback, int lane) {
+    const int grp = lane >> 3, g = lane & 7;
+    int c_n = (grp < n) ? __ldg(adj + e0 + grp) : fallback;
+    for (int i0 = 0; i0 < n; i0 += 4) {
+        const int i = i0 + grp;
+        const int c = c_n;
+        c_n = (i + 4 < n) ? __ldg(adj + e0 + i + 4) : fallback;
+        const float b = __ldg(bias + c);
+        const float s = wide_dot(s_row, emb + (size_t)c * (size_t)ld + 4 * g, g);
+        if (g == 0 && i < n) out[i] = __fadd_rn(s, b);
+    }
+    __syncwarp();
+}
+
 // max over sc[0..n)
 __device__ __forceinline__ float list_max(const float *sc, int n, int lane) {
     float m = -INFINITY;

@@ -19,6 +19,7 @@ import numpy as np
 from . import _cabi
 from ._cabi import ptr
 from .model import MAX_BATCH
+from .sampler import LD_MAX
 
 
 def block_range(n, rank, world):
@@ -119,7 +120,8 @@ class DataParallelStep:
         over NVLink (CUDA IPC mapped) and the merge kernel waits on flags -- no collective call.  Same results bit for bit."""
         assert transport in ("nccl", "p2p")
         if transport == "p2p" and DataParallelStep._p2p_capacity == 0:
-            cap_floats = self.world * int(self.lib.gg_grad_buf_floats(2 * (-(-256 // self.world)), 256))   # batches up to 256 pairs, ld 256
+            # batches up to 256 pairs at any row stride (ld up to LD_MAX)
+            cap_floats = self.world * int(self.lib.gg_grad_buf_floats(2 * (-(-256 // self.world)), LD_MAX))
             connect_peer_memory(self.comm, cap_floats, self.group)
             DataParallelStep._p2p_capacity = cap_floats
         self.transport = transport

@@ -19,18 +19,22 @@ CNT = dict(steps=0, sum_l=1, accepted=2, ok_roots=3, path_overflow=4, raw_steps=
            rows_gathered=8, cyc_enum=9, cyc_score=10, cyc_choose=11, cyc_step0=12, cyc_step1=13, cyc_step2p=14, cyc_walk=15)
 
 
+LD_MAX = 512   # widest row stride the kernels accept (gg::ld_supported in csrc/gg_common.cuh)
+
+
 def round_up(x, m):
     return (x + m - 1) // m * m
 
 
 def pad_embedding(emb, device=None):
-    """float64/32 [N, d] -> fp32 [N, ld] device tensor, ld = 32 * 2^k >= d (32, 64, 128 or 256), zero padded
+    """float64/32 [N, d] -> fp32 [N, ld] device tensor, ld = 32 * 2^k >= d (32, 64, 128, 256 or 512), zero padded
     (the tf fp32 variable of generator.py:11-14 in the HBM layout of DESIGN.md section 2)."""
     import torch
     e = emb.float() if isinstance(emb, torch.Tensor) else torch.as_tensor(np.asarray(emb, np.float64).astype(np.float32))
     n, d = e.shape
-    if d > 256:
-        raise ValueError("n_emb = %d is not supported (the kernels are instantiated for row strides 32, 64, 128, 256)" % d)
+    if d > LD_MAX:
+        raise ValueError("n_emb = %d is not supported: at most %d (the kernels are instantiated for row strides 32, 64, 128, "
+                         "256 and 512)" % (d, LD_MAX))
     ld = 32
     while ld < d:      # zero columns add exactly +0 to every canonical dot, so the amount of padding is invisible
         ld *= 2

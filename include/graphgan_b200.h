@@ -14,8 +14,8 @@
  *     synchronisation, no allocation.  Scratch is caller supplied (query *_scratch_bytes).
  *   - return 0 on success, non-zero on CUDA / argument error; gg_last_error() gives the
  *     message for the calling thread.  Nothing aborts.
- *   - embedding rows are fp32 [N, ld], zero padded, with ld = 32, 64, 128 or 256 (the smallest that holds n_emb):
- *     every entry point that takes ld rejects other values.
+ *   - embedding rows are fp32 [N, ld], zero padded, with ld = 32, 64, 128, 256 or 512 (the smallest that holds
+ *     n_emb, so n_emb <= 512): every entry point that takes ld rejects other values.
  *   - graph = two CSRs in the reference's adjacency-file order (src/utils.py:27-37):
  *       raw  : graph[i] as read (duplicates and self-loops kept) -> positives, sample_num
  *       walk : first occurrences only, self-loops dropped        -> BFS trees and walks
@@ -61,7 +61,7 @@ int gg_abi_version(void);
  * ------------------------------------------------------------------------------------------ */
 typedef struct gg_walk_desc {
     int64_t n_node;
-    int32_t ld;                 /* row stride in floats, multiple of 32 */
+    int32_t ld;                 /* row stride in floats: 32, 64, 128, 256 or 512 (see Conventions) */
     const float *emb;           /* device [N, ld]  generator.embedding_matrix (generator.py:11-14) */
     const float *bias;          /* device [N]      generator.bias_vector      (generator.py:15)    */
     const int64_t *indptr;      /* device [N+1]    walk CSR */

@@ -1,8 +1,9 @@
 """Large mini-batch benchmark of one optimizer step (K2 gradient + K3 dense Adam sweep) at the C3 shape.
 
-usage: python tools/bench_large_batch.py [--out FILE.jsonl] [--n 1000000] [--seconds 1.0] [--profile]
+usage: python tools/bench_large_batch.py [--out FILE.jsonl] [--n 1000000] [--n-emb 128] [--seconds 1.0] [--profile]
 
-Workload: N = 1M nodes, n_emb = 128 (ld 128), D-shaped rows -- the centres of synth.power_law(N, 20), each repeated
+Workload: N = 1M nodes, n_emb = 128 (ld 128; --n-emb takes another row stride: 32, 64, 128, 256 or 512),
+D-shaped rows -- the centres of synth.power_law(N, 20), each repeated
 2 * deg times, with its adjacency twice as neighbours and labels 1 then 0 (~40 M rows, grouped by centre like the rows a
 D pass emits).  For every B it times, with CUDA events over >= --seconds of work after a warm-up, on batches at random
 slice starts (always including slice 0, which holds the largest hub):
@@ -77,6 +78,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None)
     ap.add_argument("--n", type=int, default=1_000_000)
+    ap.add_argument("--n-emb", type=int, default=128, choices=[32, 64, 128, 256, 512], help="embedding width (= the row stride)")
     ap.add_argument("--seconds", type=float, default=1.0)
     ap.add_argument("--batches", default="64,1024,4096,16384,65536")
     ap.add_argument("--profile", action="store_true")
@@ -93,7 +95,7 @@ def main():
     dev = torch.device("cuda:0")
     info = card()
     emit(dict(info, kind="card"))
-    n, d = args.n, 128
+    n, d = args.n, args.n_emb
     centre, neigh, label, max_deg = d_rows(n)
     M = int(centre.shape[0])
     emit({"kind": "workload", "n": n, "n_emb": d, "rows": M, "max_degree": max_deg})
@@ -187,7 +189,7 @@ def main():
                     t = getattr(e, "device_time_total", None) or getattr(e, "cuda_time_total", 0)
                     name = e.key
                     for tag in ("mc_forward", "mc_count", "mc_number", "mc_keys", "mc_hist", "mc_scatter", "mc_terms",
-                                "mc_short_sums", "mc_long_sums", "exclusive_scan", "fill", "elementwise", "Memset"):
+                                "mc_short_sums", "mc_long_sums", "mc_long_bias", "exclusive_scan", "fill", "elementwise", "Memset"):
                         if tag in name:
                             name = tag
                             break
