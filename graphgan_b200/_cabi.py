@@ -9,7 +9,7 @@ import os
 from . import _build
 
 _LIB = None
-ABI_VERSION = 5      # == GG_ABI_VERSION of include/graphgan_b200.h
+ABI_VERSION = 6     # == GG_ABI_VERSION of include/graphgan_b200.h
 
 
 class GGError(RuntimeError):
@@ -43,7 +43,7 @@ _P, _I32, _I64, _F = C.c_void_p, C.c_int32, C.c_int64, C.c_float
 SIGNATURES = {
     "gg_last_error": (C.c_char_p, []),
     "gg_abi_version": (C.c_int, []),
-    "gg_hub_scores": (C.c_int, [_I64, _P, _P, _I32, _P, _P, _P, _P, _I32, _P, _P]),
+    "gg_hub_scores": (C.c_int, [_I64, _P, _P, _P, _P, _I32, _P, _P]),
     "gg_root_cdf": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _P]),
     "gg_walk_scratch_bytes": (C.c_int, [_I32, C.POINTER(_I64)]),
     "gg_walk_flat_bytes": (C.c_int, [_I64, _I32, _I32, C.POINTER(_I64)]),

@@ -3,9 +3,10 @@
 // The reference recomputes E.E^T + b for EVERY root (graph_gan.py:238) and re-derives the same
 // root-step softmax for each of the root's sample_num walks (:260-262).  Two exact reuses:
 //
-//  * hub_score_kernel: all_score[u, v] for the adjacency of high-degree nodes u.  A score does
+//  * hub_score_tm_kernel: all_score[u, v] for the adjacency of high-degree nodes u.  A score does
 //    not depend on the root, only the candidate SET does (children of u in that root's tree),
-//    so one pass over a hub's neighbour rows serves every walk that ever stands on u.
+//    so one pass over a hub's neighbour rows serves every walk that ever stands on u.  The pass
+//    runs target-major: each target row is read once, the (few, L2-resident) hub rows many times.
 //  * root_cdf_kernel: the root step's candidate list is tree[root][1:] = all neighbours of the
 //    root for every walk of that root, so its normalised CDF is built once per root and each
 //    walk only draws u and inverts it (walk.cu: cdf_search).
@@ -23,26 +24,40 @@ __device__ __forceinline__ float *hub_wide_row() {
     return reinterpret_cast<float *>(hub_smem + (size_t)(threadIdx.x >> 5) * WIDE_ROW_BYTES);
 }
 
+// ld = 512, target-major hub scores: the 8-lane group's target row (4 per warp)
+__device__ __forceinline__ float *hub_group_row(int grp) {
+    extern __shared__ __align__(16) unsigned char hub_smem[];
+    return reinterpret_cast<float *>(hub_smem + (size_t)(4 * (threadIdx.x >> 5) + grp) * WIDE_ROW_BYTES);
+}
+
+// CTAs per SM the kernel is compiled for: as many as the source-major kernel's registers allowed (ld 512: shared memory)
+constexpr int hub_tm_min_ctas(int cpl) { return cpl <= 2 ? 5 : cpl == 4 ? 4 : 3; }
+
+// Target-major: item t = (v, first, count, -) covers pairs[first, first + count), hub entries e = (u -> v) of ONE target v
+// stored as (u, e) (graph.py: DeviceGraph.hub_tiles).  Each 8-lane group takes one item: E[v] is read from DRAM once
+// per pass for all of v's hub entries, and the hub rows E[u] -- a few MB for all hubs together, touched by every SM all
+// the time -- stream past it from L2.  Source-major (a hub's row held, its targets gathered) read each target row once
+// per hub that lists it.
 template <int CPL>
-__global__ void __launch_bounds__(WARPS_PER_CTA * 32)
-hub_score_kernel(long long n_tiles, const int *__restrict__ tile_node, const long long *__restrict__ tile_begin,
-                 int tile_edges, const long long *__restrict__ indptr, const int *__restrict__ adj,
-                 const float *__restrict__ emb, const float *__restrict__ bias, int ld, float *__restrict__ edge_score) {
-    const int lane = threadIdx.x & 31;
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, hub_tm_min_ctas(CPL))
+hub_score_tm_kernel(long long n_items, const int4 *__restrict__ items, const int2 *__restrict__ pairs,
+                    const float *__restrict__ emb, const float *__restrict__ bias, int ld, float *__restrict__ edge_score) {
+    const int lane = threadIdx.x & 31, grp = lane >> 3;
     const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-    for (long long t = warp; t < n_tiles; t += nwarps) {
-        const int u = tile_node[t];
-        const long long e0 = tile_begin[t], a1 = indptr[u + 1];
-        const int n = (int)((a1 - e0) < tile_edges ? (a1 - e0) : tile_edges);
+    for (long long t0 = 4 * warp; t0 < n_items; t0 += 4 * nwarps) {   // (t0: warp-uniform)
+        const int4 it = (t0 + grp < n_items) ? __ldg(items + t0 + grp) : make_int4(0, 0, 0, 0);
+        const int v = it.x, n = it.z;
+        const int n_warp = __reduce_max_sync(FULL, n);
+        const float bv = __ldg(bias + v);
         if constexpr (CPL == WIDE_CPL) {
-            float *s_row = hub_wide_row();
-            load_row_wide(emb, ld, u, s_row, lane);
-            score_edges_wide(emb, bias, ld, s_row, adj, e0, n, edge_score + e0, u, lane);
+            float *s_row = hub_group_row(grp);
+            load_row_group_wide(emb, ld, v, s_row, lane & 7);
+            score_pairs_wide(emb, ld, s_row, bv, pairs + it.y, n, n_warp, edge_score, v, lane);
         } else {
             float4 c4[CPL];
-            load_row<CPL>(emb, ld, u, lane & 7, c4);
-            score_edges<CPL>(emb, bias, ld, c4, adj, e0, n, edge_score + e0, u, lane);
+            load_row<CPL>(emb, ld, v, lane & 7, c4);
+            score_pairs<CPL>(emb, ld, c4, bv, pairs + it.y, n, n_warp, edge_score, v, lane);
         }
     }
 }
@@ -77,27 +92,33 @@ root_cdf_kernel(const __grid_constant__ gg_walk_desc d, float *__restrict__ root
     }
 }
 
-// dynamic shared memory of a launch (only ld = 512 keeps the current row there)
+// dynamic shared memory of a root_cdf_kernel launch (only ld = 512 keeps the current row there)
 constexpr int hub_smem_bytes(int cpl) { return cpl == WIDE_CPL ? WARPS_PER_CTA * WIDE_ROW_BYTES : 0; }
+// ... and of a hub_score_tm_kernel launch (one row per group)
+constexpr int hub_tm_smem_bytes(int cpl) { return cpl == WIDE_CPL ? 4 * WARPS_PER_CTA * WIDE_ROW_BYTES : 0; }
 
 }  // namespace
 }  // namespace gg
 
-extern "C" int gg_hub_scores(int64_t n_tiles, const int32_t *tile_node, const int64_t *tile_begin, int32_t tile_edges,
-                             const int64_t *indptr, const int32_t *adj, const float *emb, const float *bias, int32_t ld,
-                             float *edge_score, void *stream) {
-    if (n_tiles == 0) return 0;
-    GG_REQUIRE(tile_node && tile_begin && indptr && adj && emb && bias && edge_score, "null pointer");
-    GG_REQUIRE(tile_edges > 0, "bad tile_edges");
+extern "C" int gg_hub_scores(int64_t n_items, const int32_t *items, const int32_t *pairs, const float *emb, const float *bias,
+                             int32_t ld, float *edge_score, void *stream) {
+    if (n_items == 0) return 0;
+    GG_REQUIRE(items && pairs && emb && bias && edge_score, "null pointer");
     GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
-    long long blocks = (n_tiles + gg::WARPS_PER_CTA - 1) / gg::WARPS_PER_CTA;
+    long long blocks = (n_items + 4 * gg::WARPS_PER_CTA - 1) / (4 * gg::WARPS_PER_CTA);
     const long long cap = (long long)gg::sm_count() * 8;
     if (blocks > cap) blocks = cap;
     cudaStream_t st = (cudaStream_t)stream;
+    const int4 *it = reinterpret_cast<const int4 *>(items);
+    const int2 *pr = reinterpret_cast<const int2 *>(pairs);
+    if (ld == 512) {
+        static_assert(gg::hub_tm_smem_bytes(gg::WIDE_CPL) > 48 * 1024, "the attribute is needed");
+        GG_CHECK(cudaFuncSetAttribute(gg::hub_score_tm_kernel<gg::WIDE_CPL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      gg::hub_tm_smem_bytes(gg::WIDE_CPL)));
+    }
 #define GG_LAUNCH(C)                                                                                           \
-    gg::hub_score_kernel<C><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, gg::hub_smem_bytes(C), st>>>(          \
-        n_tiles, tile_node, (const long long *)tile_begin, tile_edges, (const long long *)indptr, adj, emb, bias, ld, \
-        edge_score)
+    gg::hub_score_tm_kernel<C><<<(unsigned)blocks, gg::WARPS_PER_CTA * 32, gg::hub_tm_smem_bytes(C), st>>>(    \
+        n_items, it, pr, emb, bias, ld, edge_score)
     switch (ld / 32) {
         case 1: GG_LAUNCH(1); break;
         case 2: GG_LAUNCH(2); break;

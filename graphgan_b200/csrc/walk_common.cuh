@@ -90,6 +90,29 @@ __device__ __forceinline__ void score_list(const float *__restrict__ emb, const 
     __syncwarp();
 }
 
+// The canonical dots of the register row c4 with rows ca and cb of emb: lane g's fma chain over its chunks g, g + 8, ...,
+// then the group's butterfly.  fma(a, b, s) rounds a * b + s once whichever operand is the register row, so the dot of
+// u and v is the same bits with either of them in c4 (score_edges holds the source, score_pairs the target).
+template <int CPL>
+__device__ __forceinline__ void dot2(const float *__restrict__ emb, int ld, const float4 (&c4)[CPL], int ca, int cb, int g,
+                                     float &sa, float &sb) {
+    const float *ra = emb + (size_t)ca * (size_t)ld + 4 * g;
+    const float *rb = emb + (size_t)cb * (size_t)ld + 4 * g;
+    float4 xa[CPL], xb[CPL];
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) xa[c] = ldg4(ra + 32 * c);
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) xb[c] = ldg4(rb + 32 * c);
+    sa = 0.0f;
+    sb = 0.0f;
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) sa = fma4(c4[c], xa[c], sa);
+#pragma unroll
+    for (int c = 0; c < CPL; ++c) sb = fma4(c4[c], xb[c], sb);
+    sa = group8_sum(sa);
+    sb = group8_sum(sb);
+}
+
 // Same, for a contiguous run of adjacency entries (ids read straight from the CSR).
 template <int CPL>
 __device__ __forceinline__ void score_edges(const float *__restrict__ emb, const float *__restrict__ bias, int ld,
@@ -103,24 +126,37 @@ __device__ __forceinline__ void score_edges(const float *__restrict__ emb, const
         const int ca = ca_n, cb = cb_n;          // (next iteration's ids in flight behind this iteration's rows, see score_list)
         ca_n = (ia + 8 < n) ? __ldg(adj + e0 + ia + 8) : fallback;
         cb_n = (ib + 8 < n) ? __ldg(adj + e0 + ib + 8) : fallback;
-        const float *ra = emb + (size_t)ca * (size_t)ld + 4 * g;
-        const float *rb = emb + (size_t)cb * (size_t)ld + 4 * g;
-        float4 xa[CPL], xb[CPL];
-#pragma unroll
-        for (int c = 0; c < CPL; ++c) xa[c] = ldg4(ra + 32 * c);
-#pragma unroll
-        for (int c = 0; c < CPL; ++c) xb[c] = ldg4(rb + 32 * c);
+        float sa, sb;
+        dot2<CPL>(emb, ld, c4, ca, cb, g, sa, sb);
         const float ba = __ldg(bias + ca), bb = __ldg(bias + cb);
-        float sa = 0.0f, sb = 0.0f;
-#pragma unroll
-        for (int c = 0; c < CPL; ++c) sa = fma4(c4[c], xa[c], sa);
-#pragma unroll
-        for (int c = 0; c < CPL; ++c) sb = fma4(c4[c], xb[c], sb);
-        sa = group8_sum(sa);
-        sb = group8_sum(sb);
         if (g == 0) {
             if (va) out[ia] = __fadd_rn(sa, ba);
             if (vb) out[ib] = __fadd_rn(sb, bb);
+        }
+    }
+    __syncwarp();
+}
+
+// score_edges the other way round (hub_score_tm_kernel): c4 holds the row of ONE target v, and the group scores the n hub
+// entries e_i = (u_i -> v) listed as pairs (u_i, e_i): out[e_i] = dot(E[u_i], E[v]) + b[v] = all_score[u_i, v].  Each
+// group has its own list (n differs between the groups), two rows in flight, the next pairs fetched behind them;
+// n_warp = the largest n of the warp keeps the group butterflies warp-uniform.
+template <int CPL>
+__device__ __forceinline__ void score_pairs(const float *__restrict__ emb, int ld, const float4 (&c4)[CPL], float bv,
+                                            const int2 *__restrict__ pairs, int n, int n_warp, float *__restrict__ out,
+                                            int fallback, int lane) {
+    const int g = lane & 7;
+    const int2 fb = make_int2(fallback, 0);
+    int2 pa_n = (0 < n) ? __ldg(pairs) : fb, pb_n = (1 < n) ? __ldg(pairs + 1) : fb;
+    for (int i0 = 0; i0 < n_warp; i0 += 2) {
+        const int2 pa = pa_n, pb = pb_n;
+        pa_n = (i0 + 2 < n) ? __ldg(pairs + i0 + 2) : fb;
+        pb_n = (i0 + 3 < n) ? __ldg(pairs + i0 + 3) : fb;
+        float sa, sb;
+        dot2<CPL>(emb, ld, c4, pa.x, pb.x, g, sa, sb);
+        if (g == 0) {
+            if (i0 < n) out[pa.y] = __fadd_rn(sa, bv);
+            if (i0 + 1 < n) out[pb.y] = __fadd_rn(sb, bv);
         }
     }
     __syncwarp();
@@ -200,6 +236,31 @@ __device__ __forceinline__ void score_edges_wide(const float *__restrict__ emb, 
         const float s = wide_dot(s_row, emb + (size_t)c * (size_t)ld + 4 * g, g);
         if (g == 0 && i < n) out[i] = __fadd_rn(s, b);
     }
+    __syncwarp();
+}
+
+// score_pairs for ld = 512: s_row = the GROUP's copy of the target row (load_row_group_wide), one hub row per iteration
+__device__ __forceinline__ void score_pairs_wide(const float *__restrict__ emb, int ld, const float *s_row, float bv,
+                                                 const int2 *__restrict__ pairs, int n, int n_warp, float *__restrict__ out,
+                                                 int fallback, int lane) {
+    const int g = lane & 7;
+    const int2 fb = make_int2(fallback, 0);
+    int2 p_n = (0 < n) ? __ldg(pairs) : fb;
+    for (int i = 0; i < n_warp; ++i) {
+        const int2 p = p_n;
+        p_n = (i + 1 < n) ? __ldg(pairs + i + 1) : fb;
+        const float s = wide_dot(s_row, emb + (size_t)p.x * (size_t)ld + 4 * g, g);
+        if (g == 0 && i < n) out[p.y] = __fadd_rn(s, bv);
+    }
+    __syncwarp();
+}
+
+// the row of `node` into an 8-lane group's row buffer (WIDE_ROW_BYTES); the group's previous scoring has finished
+__device__ __forceinline__ void load_row_group_wide(const float *__restrict__ emb, int ld, int node, float *s_row, int g) {
+    const float *crow = emb + (size_t)node * (size_t)ld;
+#pragma unroll
+    for (int k = 0; k < WIDE_CPL; ++k)    // 128 float4 chunks, 16 per lane
+        *reinterpret_cast<float4 *>(s_row + 4 * (g + 8 * k)) = ldg4(crow + 4 * (g + 8 * k));
     __syncwarp();
 }
 

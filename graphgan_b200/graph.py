@@ -13,6 +13,11 @@ import numpy as np
 
 from . import _cabi
 
+# Entries per work item of the hub score pass.  A target's hub entries run 4.8 long on average at the benchmarked power
+# law (p99 34, longest 2 407): the cap keeps one target from becoming the launch's tail, and bounds how long the other
+# three 8-lane groups of a warp wait on the longest item among them.
+HUB_ITEM_CAP = 32
+
 
 def read_edge_file(path):
     """src/utils.py:50-54: whitespace separated integer pairs, one edge per line."""
@@ -123,21 +128,39 @@ class DeviceGraph:
             self._rev = rev if int(missing.item()) == 0 else None
         return self._rev
 
-    def hub_tiles(self, threshold, tile_edges=256):
-        """Work list of gg_hub_scores: (node, first entry) of every `tile_edges`-entry slice of the
-        adjacency of nodes whose walk-CSR degree is >= threshold.  Static per graph; cached."""
+    def hub_tiles(self, threshold, item_cap=HUB_ITEM_CAP):
+        """Work list of gg_hub_scores, target-major: the walk-CSR entries e = (u -> v) of the nodes u whose degree is
+        >= threshold, stably sorted by target v, as pairs (u, e) (device int32 [n_entries, 2]), and the work items
+        (v, first pair, count, 0) (device int32 [n_items, 4]) that cut each target's run of pairs into pieces of at most
+        `item_cap`.  Returns (items, pairs, n_items, n_entries).  Built on the device; static per graph; cached."""
         import torch
-        key = (int(threshold), int(tile_edges))
+        key = (int(threshold), int(item_cap))
         if getattr(self, "_hub_key", None) != key:
-            deg = np.diff(self.host.indptr)
-            hubs = np.flatnonzero(deg >= threshold)
-            nt = (deg[hubs] + tile_edges - 1) // tile_edges
-            node = np.repeat(hubs, nt).astype(np.int32)
-            first = np.repeat(np.cumsum(nt) - nt, nt)
-            begin = (self.host.indptr[node] + (np.arange(node.shape[0]) - first) * tile_edges).astype(np.int64)
+            dev, i64 = self.device, torch.int64
+            deg_h = np.diff(self.host.indptr)
+            hubs_h = np.flatnonzero(deg_h >= threshold)
+            n_entries = int(deg_h[hubs_h].sum())
+            items = torch.zeros((0, 4), dtype=torch.int32, device=dev)
+            pairs = torch.zeros((0, 2), dtype=torch.int32, device=dev)
+            if n_entries:
+                hubs = torch.from_numpy(hubs_h).to(dev)
+                cnt = self.indptr[hubs + 1] - self.indptr[hubs]
+                src = torch.repeat_interleave(hubs, cnt, output_size=n_entries)                  # hub-major order
+                run0 = torch.repeat_interleave(torch.cumsum(cnt, 0) - cnt, cnt, output_size=n_entries)
+                e = self.indptr[src] + (torch.arange(n_entries, dtype=i64, device=dev) - run0)
+                tgt, order = torch.sort(self.adj[e], stable=True)
+                pairs = torch.stack([src[order], e[order]], 1).to(torch.int32).contiguous()
+                v, run = torch.unique_consecutive(tgt, return_counts=True)
+                pieces = (run + item_cap - 1) // item_cap
+                n_items = int(pieces.sum().item())
+                p0 = torch.cumsum(pieces, 0) - pieces                                            # first piece of each run
+                r = torch.repeat_interleave(torch.arange(v.shape[0], dtype=i64, device=dev), pieces, output_size=n_items)
+                k = torch.arange(n_items, dtype=i64, device=dev) - p0[r]                         # piece index in its run
+                first = (torch.cumsum(run, 0) - run)[r] + k * item_cap
+                count = torch.clamp(run[r] - k * item_cap, max=item_cap)
+                items = torch.stack([v[r].to(i64), first, count, torch.zeros_like(first)], 1).to(torch.int32).contiguous()
             self._hub_key = key
-            self._hub = (torch.from_numpy(node).to(self.device), torch.from_numpy(begin).to(self.device),
-                         int(node.shape[0]), int(deg[hubs].sum()))
+            self._hub = (items, pairs, int(items.shape[0]), n_entries)
             if not hasattr(self, "edge_score"):
                 self.edge_score = torch.empty(self.host.adj.shape[0] + 4, dtype=torch.float32, device=self.device)[:max(self.host.adj.shape[0], 1)]
         return self._hub

@@ -272,10 +272,10 @@ class WalkSampler:
         embeddings, so it belongs to every pass; `run` calls it unless told otherwise."""
         d = desc if desc is not None else self._desc(emb, bias, plan, seed=0, pass_tag=0, update_ratio=1.0,
                                                      rng_mode=RNG_PHILOX, stream=None, reuse=True)
-        tile_node, tile_begin, n_tiles, _ = self.g.hub_tiles(self.hub_threshold)
+        items, pairs, n_items, _ = self.g.hub_tiles(self.hub_threshold)
         st = self._stream()
-        _cabi.check(self.lib.gg_hub_scores(n_tiles, ptr(tile_node), ptr(tile_begin), 256, ptr(self.g.indptr), ptr(self.g.adj),
-                                           ptr(emb), ptr(bias), int(emb.shape[1]), ptr(self.g.edge_score), st), "gg_hub_scores")
+        _cabi.check(self.lib.gg_hub_scores(n_items, ptr(items), ptr(pairs), ptr(emb), ptr(bias), int(emb.shape[1]),
+                                           ptr(self.g.edge_score), st), "gg_hub_scores")
         _cabi.check(self.lib.gg_root_cdf(C.byref(d), ptr(plan.root_sc), ptr(plan.root_q), st), "gg_root_cdf")
 
     def run(self, emb, bias, trees, sample_num, for_d, *, seed=0, pass_tag=0, update_ratio=1.0, max_path=0,

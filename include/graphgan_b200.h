@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 5
+#define GG_ABI_VERSION 6
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -138,12 +138,12 @@ typedef struct gg_walk_desc {
     int32_t flat_reserved;
 } gg_walk_desc;
 
-/* all_score[u, v] = e_u.e_v + b_v (generator.py:21) for every walk-CSR entry (u -> v) of the listed hub
- * tiles: tile t covers entries [tile_begin[t], min(tile_begin[t] + tile_edges, indptr[tile_node[t]+1])).
- * Must be re-run whenever the generator's embeddings change (i.e. once per sampling pass). */
-int gg_hub_scores(int64_t n_tiles, const int32_t *tile_node, const int64_t *tile_begin, int32_t tile_edges,
-                  const int64_t *indptr, const int32_t *adj, const float *emb, const float *bias, int32_t ld,
-                  float *edge_score, void *stream);
+/* all_score[u, v] = e_u.e_v + b_v (generator.py:21) for the listed walk-CSR entries e = (u -> v), grouped by
+ * target: pairs = device int32 [n_pairs, 2] of (u, e), items = device int32 [n_items, 4] of (v, first, count, unused),
+ * item t covering pairs[first, first + count), all of them entries into v; edge_score[e] is written for every listed
+ * pair.  Must be re-run whenever the generator's embeddings change (i.e. once per sampling pass). */
+int gg_hub_scores(int64_t n_items, const int32_t *items, const int32_t *pairs, const float *emb, const float *bias,
+                  int32_t ld, float *edge_score, void *stream);
 /* Root-step softmax + CDF, once per root per pass: root_q[rq_ptr[k] + i] = cdf_i / cdf_last over the
  * candidates tree[root][1:] (graph_gan.py:250,260-262).  Uses d->{roots, n_roots, indptr, adj, emb, bias,
  * ld, rq_ptr, edge_score, hub_threshold}.  root_sc: device float scratch of rq_ptr[R] entries. */

@@ -17,7 +17,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-FAMILIES = ["hub_score_kernel", "root_cdf_kernel", "root_step_kernel", "step1_cdf_kernel", "flat_start_kernel", "flat_enum_kernel",
+FAMILIES = ["hub_score_tm_kernel", "root_cdf_kernel", "root_step_kernel", "step1_cdf_kernel", "flat_start_kernel", "flat_enum_kernel",
             "flat_choose_kernel", "walk_kernel", "finalize_kernel",
             "emit_rows_kernel", "bfs_kernel", "adam_kernel", "reward_kernel", "pair_grad_kernel"]
 
@@ -56,7 +56,7 @@ def main():
     if doc.get("source_hash") != h:
         doc = {"source_hash": h, "kernels": {}, "detail": {}}
     walk = ["flat_start_kernel", "flat_enum_kernel", "flat_choose_kernel", "walk_kernel"]   # the walk stage (one walk_kernel per pass)
-    k1 = ["hub_score_kernel", "root_cdf_kernel", "root_step_kernel", "step1_cdf_kernel"] + walk
+    k1 = ["hub_score_tm_kernel", "root_cdf_kernel", "root_step_kernel", "step1_cdf_kernel"] + walk
     entry = {f: per[f]["dram_bytes"] / per[f]["launches"] for f in per}
     if "walk_kernel" in per:
         passes = per["walk_kernel"]["launches"]             # the capture must cover whole passes
@@ -66,7 +66,7 @@ def main():
             if f in per:
                 entry[f + "_per_pass"] = per[f]["dram_bytes"] / passes
                 entry[f + "_ncu_us_per_pass"] = per[f]["time_ns"] / passes / 1e3
-        if all(f in per for f in ("hub_score_kernel", "root_cdf_kernel")):
+        if all(f in per for f in ("hub_score_tm_kernel", "root_cdf_kernel")):
             entry["k1_stage"] = sum(per[f]["dram_bytes"] for f in k1 if f in per) / passes
     doc["kernels"].setdefault(key, {}).update(entry)
     doc["detail"].setdefault(key, {}).update({f: {"launches": per[f]["launches"], "dram_bytes_per_launch": entry[f],

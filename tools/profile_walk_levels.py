@@ -10,7 +10,9 @@ torch.profiler (CUDA activities only) for --passes passes and writes ONE JSON re
               keys (distinct (root slot, node) items of a shared level that are not score-cached; 0 on a level that
               does not share) and hub owners / hub work items (distinct score-cached (root slot, node) groups of a
               shared level and the work items they were split into; 0 where hub walks run per walk);
-  stage       flat_start_kernel, the walk_kernel tail, and the whole walk stage (first to last of its kernels).
+  stage       flat_start_kernel, the walk_kernel tail, and the whole walk stage (first to last of its kernels);
+  precompute  device microseconds per pass of the per-pass precompute kernels (the hub score kernel and root_cdf_kernel),
+              from a second profiled region of --passes whole passes of its own.
 
 The levels reuse kernel names, so a kernel is given to a level by launch order within the pass.  Load an A/B library
 with GG_LIB=<path> (tools/variants.py) to profile another build.
@@ -79,6 +81,20 @@ def split_levels(events, n_passes):
     return passes
 
 
+def precompute_kernels(events, n_passes):
+    """{kernel: microseconds per pass} of the precompute kernels (hub_score*_kernel, root_cdf_kernel)"""
+    tot, cnt = {}, {}
+    for _, dur, name in events:
+        base = name.split("<")[0]
+        if base.startswith("hub_score") or base == "root_cdf_kernel":
+            tot[name] = tot.get(name, 0) + dur
+            cnt[name] = cnt.get(name, 0) + 1
+    for k, c in cnt.items():
+        if c != n_passes:
+            raise RuntimeError("found %d launches of %s in the trace, expected %d" % (c, k, n_passes))
+    return {k: round(v / n_passes / 1e3, 2) for k, v in sorted(tot.items())}
+
+
 def gpu_info():
     try:
         r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
@@ -141,7 +157,12 @@ def main():
             ctrs.append(plan._flat[:4 * FLAT_CTR_ALL].clone())        # device copy, read after the region
         torch.cuda.synchronize()
     passes = split_levels(kernel_events(prof), args.passes)
-    ctr = np.stack([c.view(torch.int32).cpu().numpy().astype(np.int64) for c in ctrs])   # [passes, words]
+    with profile(activities=[ProfilerActivity.CUDA]) as prof_pre:     # precompute: a region of its own
+        for s in range(args.passes):
+            one_pass(3000 + s)
+        torch.cuda.synchronize()
+    pre = precompute_kernels(kernel_events(prof_pre), args.passes)
+    ctr =np.stack([c.view(torch.int32).cpu().numpy().astype(np.int64) for c in ctrs])   # [passes, words]
 
     levels = {}
     for s in range(1, smp.flat_steps + 1):
@@ -164,7 +185,9 @@ def main():
         "tail_records": int(ctr[:, 0].mean()),
         "walk_stage_span_us": round(float(np.mean([sp[1] - sp[0] for _, sp in passes])) / 1e3, 2),
         "walk_stage_kernel_sum_us": round(float(np.mean([sum(sum(v.values()) for v in per.values()) for per, _ in passes])) / 1e3, 2),
-        "note": "device time per pass (mean over the profiled passes); span = first walk-stage kernel start to the tail's "
+        "precompute_us": pre, "precompute_total_us": round(sum(pre.values()), 2),
+        "hub_entries": int(dg.hub_tiles(smp.hub_threshold)[3]),
+        "note":"device time per pass (mean over the profiled passes); span = first walk-stage kernel start to the tail's "
                 "end, kernel_sum = the sum of the stage's kernel durations (the gaps between them are the difference)",
     }
     line = json.dumps(rec)
