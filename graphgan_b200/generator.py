@@ -34,3 +34,25 @@ class Generator(PairModel):
     def g_step(self, node_id, node_neighbor_id, reward):
         """sess.run(generator.g_updates, {node_id, node_neighbor_id, reward}) (graph_gan.py:173-176)."""
         self.step(node_id, node_neighbor_id, reward)
+
+    def relevance(self, roots, nodes=None, sampler=None):
+        """G(v | root) of the current generator: the exact probability that one generator walk from the root stops at v
+        (csrc/gdist.cu, DESIGN.md section 5.1), under the graph's current father-removal bits.  ``sampler``: the
+        sampler.WalkSampler of the graph (default: the one GraphGAN attaches as ``self.sampler``).
+        nodes=None: device fp64 rows [len(roots), N]; otherwise ``nodes`` pairs with ``roots`` element by element and the
+        result is dist[root_k, nodes_k] (fp64 [len(roots)]).  A root whose walks void has an all-zero row."""
+        import numpy as np
+        torch = self.torch
+        smp = sampler if sampler is not None else getattr(self, "sampler", None)
+        if smp is None:
+            raise ValueError("relevance needs the graph's WalkSampler (pass sampler=...)")
+        r = np.asarray(roots.cpu() if isinstance(roots, torch.Tensor) else roots, np.int64).reshape(-1)
+        if nodes is None:
+            dist, _ = smp.distribution(self.emb, self.bias_t, smp.build_trees(r.astype(np.int32)))
+            return dist
+        v = torch.as_tensor(np.asarray(nodes.cpu() if isinstance(nodes, torch.Tensor) else nodes, np.int64).reshape(-1))
+        if v.shape[0] != r.shape[0]:
+            raise ValueError("roots and nodes must have the same length")
+        uniq, inv = np.unique(r, return_inverse=True)
+        dist, _ = smp.distribution(self.emb, self.bias_t, smp.build_trees(uniq.astype(np.int32)))
+        return dist[torch.as_tensor(inv).to(dist.device), v.to(dist.device)]

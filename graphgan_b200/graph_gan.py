@@ -103,6 +103,7 @@ class GraphGAN(object):
 
     def build_generator(self):
         self.generator = Generator(n_node=self.n_node, node_emd_init=self.node_embed_init_g, device=self.device)
+        self.generator.sampler = self.sampler     # Generator.relevance: G(v | root) over this graph's BFS trees
 
     def build_discriminator(self):
         self.discriminator = Discriminator(n_node=self.n_node, node_emd_init=self.node_embed_init_d, device=self.device)

@@ -301,6 +301,47 @@ class WalkSampler:
             self.finalize(out)
         return out
 
+    # ------------------------------------------------------------------ exact generator distribution
+    def distribution(self, emb, bias, trees, *, reuse=None, max_scratch_bytes=None, counters=None):
+        """G(v | root) for every root of ``trees``: the exact probability that one G-mode walk (graph_gan.py:225-270)
+        from the root stops at v, under the current father-removal bits (csrc/gdist.cu, DESIGN.md section 5.1).
+        Returns device fp64 ``dist [R, N]`` and int32 ``root_ok [R]`` (0: the root's walks void; its row is all zero).
+        ``reuse`` (default: hub_threshold > 0) scores hub lists from the per-pass cache -- the same bits either way.  The
+        roots run in chunks whose scratch stays within ``max_scratch_bytes`` (default 2 GiB, env GG_GDIST_SCRATCH);
+        ``counters`` (optional device int64 [16]) receives the embedding rows fetched in slot rows_gathered."""
+        torch, g = self.torch, self.g
+        assert emb.dtype == torch.float32 and emb.is_contiguous() and bias.dtype == torch.float32
+        R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
+        dist = torch.empty((R, N), dtype=torch.float64, device=self.device)
+        root_ok = torch.empty(R, dtype=torch.int32, device=self.device)
+        if R == 0:
+            return dist, root_ok
+        reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
+        budget = int(max_scratch_bytes if max_scratch_bytes is not None else os.environ.get("GG_GDIST_SCRATCH", 2 << 30))
+
+        def scratch_bytes(k):
+            nb = C.c_int64(0)
+            _cabi.check(self.lib.gg_generator_dist_scratch_bytes(N, nnz, k, C.byref(nb)), "gg_generator_dist_scratch_bytes")
+            return nb.value
+        chunk = max(1, min(R, budget // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
+        d = _cabi.WalkDesc()
+        d.n_node, d.ld = N, int(emb.shape[1])
+        d.emb, d.bias, d.indptr, d.adj = ptr(emb), ptr(bias), ptr(g.indptr), ptr(g.adj)
+        d.tree_words, d.d1_bits, d.counters = int(trees.tree_bits.shape[1]), ptr(g.d1_bits), ptr(counters)
+        st = self._stream()
+        if reuse:
+            items, pairs, n_items, _ = g.hub_tiles(self.hub_threshold)
+            _cabi.check(self.lib.gg_hub_scores(n_items, ptr(items), ptr(pairs), ptr(emb), ptr(bias), int(emb.shape[1]),
+                                               ptr(g.edge_score), st), "gg_hub_scores")
+            d.edge_score, d.hub_threshold = ptr(g.edge_score), self.hub_threshold
+        for lo in range(0, R, chunk):
+            hi = min(R, lo + chunk)
+            d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(trees.roots[lo:hi]), ptr(trees.tree_bits[lo:hi])
+            _cabi.check(self.lib.gg_generator_dist(C.byref(d), ptr(dist[lo:hi]), ptr(root_ok[lo:hi]), ptr(scratch),
+                                                   scratch.numel(), st), "gg_generator_dist")
+        return dist, root_ok
+
     def finalize(self, out):
         _cabi.check(self.lib.gg_walk_finalize(out.n_roots, ptr(out.walk_ptr), int(out.for_d), ptr(out.samples),
                                               ptr(out.status), ptr(out.first_edge), ptr(out.wsteps), ptr(out.wsuml),

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 6
+#define GG_ABI_VERSION 7
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -161,6 +161,23 @@ int gg_walk_finalize(int64_t n_roots, const int64_t *walk_ptr, int32_t for_d, in
                      int32_t *status, const int32_t *first_edge, int32_t *wsteps, int32_t *wsuml,
                      int32_t *path_len, uint32_t *d1_bits, int32_t *root_ok,
                      unsigned long long *counters, void *stream);
+
+/* The exact generator distribution G(v | root) (csrc/gdist.cu, DESIGN.md section 5.1): for every root k of the batch,
+ * dist[k, v] = the probability that one G-mode walk from roots[k] (graph_gan.py:225-270, for_d = 0) stops at v, computed
+ * from the walk's own candidate lists and canonical CDFs in fp64 -- not sampled.  Step law of a list with canonical CDF q:
+ * pi(x_j) = (ceil(q_j 2^53) - ceil(q_{j-1} 2^53)) / 2^53; reach(root) = 1, reach(child) = reach(a) * pi_a(child),
+ * dist[k, v] = reach(v) * pi_v(father(v)), each one fixed chain of fp64 products (bit-reproducible).  dist[k, root] = 0 and
+ * dist = 0 off the tree.  root_ok[k] = 1 when the walks of the root cannot void (the root has children, and no reachable
+ * depth-1 node whose father entry is removed has an empty list); root_ok[k] = 0 rows are all zero.
+ * Uses d->{n_node, ld, emb, bias, indptr, adj, n_roots, roots, tree_bits, tree_words, d1_bits (NULL: no father entry
+ * removed), edge_score + hub_threshold (optional: cached scores of nodes with degree >= hub_threshold, gg_hub_scores; the
+ * same bits either way)} and adds the embedding rows it fetches to d->counters[GG_CNT_ROWS_GATHERED] when counters is set;
+ * the walk fields are ignored.  dist: device fp64 [n_roots, n_node]; root_ok: device [n_roots]; n_roots * n_node < 2^31.
+ * scratch: device, at least gg_generator_dist_scratch_bytes(n_node, nnz, n_roots) bytes (host-only size computation;
+ * O(n_roots * (nnz + n_node))).  One cooperative launch. */
+int gg_generator_dist_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int64_t *bytes);
+int gg_generator_dist(const gg_walk_desc *d, double *dist, int32_t *root_ok, void *scratch, int64_t scratch_bytes,
+                      void *stream);
 
 /* prepare_data_for_d's output rows (graph_gan.py:192-201): for every accepted root, in batch
  * order: [i]*k + [i]*k | pos + neg | 1*k + 0*k.  row_ptr: device [R+1] scratch/out (exclusive
