@@ -56,3 +56,5 @@ max_path_len = 64                   # row stride of recorded generator paths; a 
 text_embeddings = True              # the reference's text dump (graph_gan.py:293-306); turn off at N >= 1e5 (minutes per epoch)
 binary_embeddings = False           # also dump <emb_filename>.f32 (header + [N, n_emb] fp32, row-major) every epoch
 device_eval = True                  # link-prediction check on the GPU (io/evaluation text round trip skipped)
+value_roots = 0                     # > 0: evaluation also writes "value:<V> pos:<..> neg:<..> roots:<n>", the exact game value
+                                    # (DESIGN.md section 5.2) averaged over this many seeded roots (rank 0's shard under torchrun)

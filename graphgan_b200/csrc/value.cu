@@ -1,0 +1,274 @@
+// value.cu -- the GraphGAN game value V_c(G, D) per root, exactly (DESIGN.md section 5.2).
+//
+//   V_c  = pos_c + neg_c
+//   pos_c = -(1 / |graph[c]|) sum_k bce(s(c, graph[c][k]), 1)      raw adjacency, entry order, duplicates and self-loops
+//   neg_c = -sum_v G(v | c) bce(s(c, v), 0)                         G(v | c): gg_generator_dist's rows (G mode)
+//   s(c, v) = __fadd_rn(canonical 8-lane dot(E_D[c], E_D[v]), b_D[v])  (fp32, the bits of reward_kernel's score)
+//   bce(s, y) = (max(s, 0) - s y) + log1p(exp(-|s|))                  (fp64 from the fp32 s; discriminator.py:26-30)
+//
+// Every sum has one fixed order, so the bits depend on the inputs only (not on the grid, the chunk of roots or the
+// order of the roots):
+//   neg: nodes in tiles of VAL_TILE; inside a tile, 8-lane group q takes nodes q, q + 32, ... (one fp64 chain each), the
+//        32 group partials of a root are added as ((q0 + q1) + (q2 + q3)) per warp (xor 8, 16) and then warp 0 .. 7 in
+//        order; value_reduce_kernel adds a root's tile partials with lane l chaining tiles l, l + 32, ... and a xor
+//        butterfly over the lanes.
+//   pos: one CTA per root (its neighbour list can be the 13 828 entries of a hub); group q chains entries q, q + 32, ...,
+//        then the same warp and CTA combination.
+#include <math.h>
+
+#include "gg_common.cuh"
+
+namespace gg {
+namespace {
+
+constexpr int VAL_THREADS = 256;                   // 8 warps = 32 8-lane groups
+constexpr int VAL_GROUPS = VAL_THREADS / 8;
+constexpr int VAL_NPG = 16;                        // nodes per group and tile
+constexpr long long VAL_TILE = VAL_GROUPS * VAL_NPG;   // 512 nodes
+// roots per root tile: their rows sit in shared memory (32 KB at ld >= 128), and each lane keeps RT / 8 fp64 sums
+__host__ __device__ constexpr int val_root_tile(int cpl) { return cpl <= 4 ? 64 : 256 / cpl; }
+__host__ __device__ constexpr size_t val_smem_bytes(int cpl) {
+    return (size_t)val_root_tile(cpl) * 32 * cpl * sizeof(float) + (size_t)(VAL_THREADS / 32) * val_root_tile(cpl) * sizeof(double);
+}
+long long val_tiles(long long n_node) { return (n_node + VAL_TILE - 1) / VAL_TILE; }
+
+struct ValArgs {
+    long long n_node, n_roots, n_tiles;
+    const float *emb, *bias;
+    const long long *raw_indptr;
+    const int *raw_adj, *roots, *root_ok;
+    const double *dist;
+    double *pos, *partial;                          // partial: [n_roots, n_tiles]
+};
+
+// bce(s, y) of TF's sigmoid_cross_entropy_with_logits, in fp64 from the fp32 logit
+__device__ __forceinline__ double bce_logits(float s, bool y) {
+    const double x = (double)s;
+    const double m = fmax(x, 0.0);
+    return __dadd_rn(y ? __dsub_rn(m, x) : m, log1p(exp(-fabs(x))));
+}
+
+__device__ __forceinline__ bool value_ok(const ValArgs &a, long long k, long long &lo, long long &deg) {
+    const int c = __ldg(a.roots + k);
+    lo = __ldg(a.raw_indptr + c);
+    deg = __ldg(a.raw_indptr + c + 1) - lo;
+    return deg > 0 && __ldg(a.root_ok + k) == 1;
+}
+
+// group8_sum of eight dots at once: lane g of the group returns dot g.  Each dot goes through group8_sum's own tree
+// (xor 4, then 2, then 1; the adds only swap operands), so the bits are the same, with 7 shuffles instead of 24.
+__device__ __forceinline__ float group8_sum8(const float (&s)[8], int g) {
+    const bool h4 = (g & 4) != 0, h2 = (g & 2) != 0, h1 = (g & 1) != 0;
+    float t[4], u[2];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {                    // t[j]: dot j + 4 h4
+        const float keep = h4 ? s[j + 4] : s[j], send = h4 ? s[j] : s[j + 4];
+        t[j] = __fadd_rn(keep, __shfl_xor_sync(FULL, send, 4));
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {                    // u[j]: dot j + 2 h2 + 4 h4
+        const float keep = h2 ? t[j + 2] : t[j], send = h2 ? t[j] : t[j + 2];
+        u[j] = __fadd_rn(keep, __shfl_xor_sync(FULL, send, 2));
+    }
+    const float keep = h1 ? u[1] : u[0], send = h1 ? u[0] : u[1];
+    return __fadd_rn(keep, __shfl_xor_sync(FULL, send, 1));
+}
+
+// ((q0 + q1) + (q2 + q3)) over the four 8-lane groups of a warp: lane g of every group returns the sum of the groups'
+// lane-g values
+__device__ __forceinline__ double warp_groups_sum(double x) {
+    x = __dadd_rn(x, __shfl_xor_sync(FULL, x, 8));
+    return __dadd_rn(x, __shfl_xor_sync(FULL, x, 16));
+}
+
+// pos_c for root slot k: one CTA
+template <int CPL>
+__device__ void pos_item(const ValArgs &a, long long k, double *s_part) {
+    constexpr int LD = 32 * CPL;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane & 7, grp = threadIdx.x >> 3;
+    long long lo, deg;
+    const bool ok = value_ok(a, k, lo, deg);          // uniform over the CTA
+    if (!ok) {
+        if (threadIdx.x == 0) a.pos[k] = 0.0;
+        return;
+    }
+    const int c = __ldg(a.roots + k);
+    float4 rc[CPL];
+#pragma unroll
+    for (int j = 0; j < CPL; ++j) rc[j] = ldg4(a.emb + (size_t)c * LD + 4 * g + 32 * j);
+    double acc = 0.0;
+#pragma unroll 4
+    for (long long e0 = 0; e0 < deg; e0 += VAL_GROUPS) {
+        const long long e = e0 + grp;
+        const bool valid = e < deg;
+        const int v = valid ? __ldg(a.raw_adj + lo + e) : c;
+        float s = 0.0f;
+#pragma unroll
+        for (int j = 0; j < CPL; ++j) s = fma4(rc[j], ldg4(a.emb + (size_t)v * LD + 4 * g + 32 * j), s);
+        s = __fadd_rn(group8_sum(s), __ldg(a.bias + v));
+        if (valid) acc = __dadd_rn(acc, bce_logits(s, true));
+    }
+    acc = warp_groups_sum(acc);
+    if (lane == 0) s_part[wid] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double x = s_part[0];
+        for (int w = 1; w < VAL_THREADS / 32; ++w) x = __dadd_rn(x, s_part[w]);
+        a.pos[k] = -__ddiv_rn(x, (double)deg);
+    }
+    __syncthreads();
+}
+
+// The tile partials of neg for root tile rt (roots rt * RT ..) and node tile t; the root rows are in s_root.
+template <int CPL>
+__device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_root, double *s_part) {
+    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL), RJ = RT / 8;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane & 7, grp = threadIdx.x >> 3;
+    const long long k0 = (long long)rt * RT;
+    double acc[RJ];
+#pragma unroll
+    for (int j = 0; j < RJ; ++j) acc[j] = 0.0;
+    for (int i = 0; i < VAL_NPG; ++i) {
+        const long long v = t * VAL_TILE + grp + (long long)VAL_GROUPS * i;
+        const bool valid = v < a.n_node;
+        const long long vv = valid ? v : 0;
+        float4 row[CPL];
+#pragma unroll
+        for (int j = 0; j < CPL; ++j) row[j] = ldg4(a.emb + (size_t)vv * LD + 4 * g + 32 * j);
+        const float bv = __ldg(a.bias + vv);
+        double w[RJ];                                // lane g weighs root k0 + 8 j + g
+#pragma unroll
+        for (int j = 0; j < RJ; ++j) {
+            const long long k = k0 + 8 * j + g;
+            w[j] = (valid && k < a.n_roots) ? __ldg(a.dist + (size_t)k * (size_t)a.n_node + (size_t)v) : 0.0;
+        }
+#pragma unroll
+        for (int j = 0; j < RJ; ++j) {
+            float s[8];
+#pragma unroll
+            for (int r = 0; r < 8; ++r) {
+                const float *rr = s_root + (8 * j + r) * LD + 4 * g;
+                float x = 0.0f;
+#pragma unroll
+                for (int c = 0; c < CPL; ++c) x = fma4(*reinterpret_cast<const float4 *>(rr + 32 * c), row[c], x);
+                s[r] = x;
+            }
+            const float sc = __fadd_rn(group8_sum8(s, g), bv);
+            if (w[j] != 0.0) acc[j] = __dadd_rn(acc[j], __dmul_rn(w[j], bce_logits(sc, false)));
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < RJ; ++j) {
+        const double x = warp_groups_sum(acc[j]);
+        if (lane < 8) s_part[wid * RT + 8 * j + lane] = x;
+    }
+    __syncthreads();
+    if (threadIdx.x < RT && k0 + threadIdx.x < a.n_roots) {
+        double x = s_part[threadIdx.x];
+        for (int w = 1; w < VAL_THREADS / 32; ++w) x = __dadd_rn(x, s_part[w * RT + threadIdx.x]);
+        a.partial[(size_t)(k0 + threadIdx.x) * (size_t)a.n_tiles + (size_t)t] = x;
+    }
+    __syncthreads();
+}
+
+// Work items: first one pos item per root (a hub root's list is the longest single item, so it starts first), then the
+// (root tile, node tile) items of neg, node tile fastest so that a CTA keeps its root rows across items.
+template <int CPL>
+__global__ void __launch_bounds__(VAL_THREADS) value_kernel(const ValArgs a) {
+    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
+    extern __shared__ __align__(16) unsigned char val_smem[];
+    float *s_root = reinterpret_cast<float *>(val_smem);                                   // [RT, LD]
+    double *s_part = reinterpret_cast<double *>(val_smem + (size_t)RT * LD * sizeof(float));   // [8 warps, RT]
+    const long long n_rt = (a.n_roots + RT - 1) / RT, n_items = a.n_roots + n_rt * a.n_tiles;
+    long long cur_rt = -1;
+    for (long long item = blockIdx.x; item < n_items; item += gridDim.x) {
+        if (item < a.n_roots) {
+            pos_item<CPL>(a, item, s_part);
+            continue;
+        }
+        const long long ni = item - a.n_roots, rt = ni / a.n_tiles, t = ni % a.n_tiles;
+        if (rt != cur_rt) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
+                const long long k = rt * RT + i / (LD / 4);
+                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
+                reinterpret_cast<float4 *>(s_root)[i] = x;
+            }
+            __syncthreads();
+            cur_rt = rt;
+        }
+        neg_item<CPL>(a, (int)rt, t, s_root, s_part);
+    }
+}
+
+// neg_c = -(sum of the root's tile partials); warp per root
+__global__ void __launch_bounds__(256) value_reduce_kernel(const ValArgs a, double *__restrict__ neg, int *__restrict__ ok) {
+    const int lane = threadIdx.x & 31;
+    const long long k = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (k >= a.n_roots) return;
+    const double *p = a.partial + (size_t)k * (size_t)a.n_tiles;
+    double x = 0.0;
+    for (long long t = lane; t < a.n_tiles; t += 32) x = __dadd_rn(x, p[t]);
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) x = __dadd_rn(x, __shfl_xor_sync(FULL, x, off));
+    if (lane == 0) {
+        long long lo, deg;
+        const bool good = value_ok(a, k, lo, deg);
+        neg[k] = good ? -x : 0.0;
+        ok[k] = good ? 1 : 0;
+    }
+}
+
+template <int CPL>
+int launch_value(const ValArgs &a, double *neg, int *ok, cudaStream_t st) {
+    const size_t smem = val_smem_bytes(CPL);
+    int per_sm = 0;
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_kernel<CPL>, VAL_THREADS, smem));
+    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
+    const long long RT = val_root_tile(CPL);
+    const long long n_items = a.n_roots + (a.n_roots + RT - 1) / RT * a.n_tiles;
+    long long grid = (long long)sm_count() * per_sm;
+    if (grid > n_items) grid = n_items;
+    value_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a);
+    GG_CHECK(cudaGetLastError());
+    value_reduce_kernel<<<(unsigned)((a.n_roots + 7) / 8), 256, 0, st>>>(a, neg, ok);
+    return check_cuda(cudaGetLastError(), "game value reduce launch");
+}
+
+}  // namespace
+}  // namespace gg
+
+extern "C" int gg_game_value_scratch_bytes(int64_t n_node, int64_t n_roots, int64_t *bytes) {
+    GG_REQUIRE(bytes && n_node >= 0 && n_roots >= 0, "bad arguments");
+    *bytes = (int64_t)(sizeof(double) * (size_t)n_roots * (size_t)gg::val_tiles(n_node));
+    return 0;
+}
+
+extern "C" int gg_game_value(int64_t n_node, int32_t ld, const float *emb, const float *bias, const int64_t *raw_indptr,
+                             const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist,
+                             const int32_t *root_ok, double *pos, double *neg, int32_t *ok, void *scratch,
+                             int64_t scratch_bytes, void *stream) {
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
+    GG_REQUIRE(n_node > 0 && n_node < (1ll << 31), "n_node must lie in [1, 2^31)");
+    GG_REQUIRE(n_roots >= 0, "n_roots must be >= 0");
+    if (n_roots == 0) return 0;
+    GG_REQUIRE(emb && bias && raw_indptr && raw_adj && roots, "null graph/embedding pointer");
+    GG_REQUIRE(dist && root_ok, "null generator distribution pointer");
+    GG_REQUIRE(pos && neg && ok && scratch, "null output or scratch pointer");
+    int64_t need = 0;
+    gg_game_value_scratch_bytes(n_node, n_roots, &need);
+    GG_REQUIRE(scratch_bytes >= need, "scratch too small (gg_game_value_scratch_bytes)");
+    gg::ValArgs a;
+    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = gg::val_tiles(n_node);
+    a.emb = emb; a.bias = bias; a.raw_indptr = (const long long *)raw_indptr; a.raw_adj = raw_adj; a.roots = roots;
+    a.root_ok = root_ok; a.dist = dist; a.pos = pos; a.partial = static_cast<double *>(scratch);
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (ld / 32) {
+        case 1: return gg::launch_value<1>(a, neg, ok, st);
+        case 2: return gg::launch_value<2>(a, neg, ok, st);
+        case 4: return gg::launch_value<4>(a, neg, ok, st);
+        case 8: return gg::launch_value<8>(a, neg, ok, st);
+        default: return gg::launch_value<16>(a, neg, ok, st);
+    }
+}

@@ -129,6 +129,50 @@ class GraphGAN(object):
         for s in range(0, roots.shape[0], config.root_batch):
             yield self.construct_trees(roots[s:s + config.root_batch])
 
+    # ------------------------------------------------------------------ the game value V(G, D) (DESIGN.md section 5.2)
+    def game_value(self, roots):
+        """V_c(G, D) = pos_c + neg_c of the current generator and discriminator for every root c of ``roots`` (Wang et al.,
+        AAAI-18, Eq. 1), exactly: sampler.WalkSampler.game_value.  Returns device (pos fp64, neg fp64, ok int32)."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        return self.sampler.game_value(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
+
+    def _trees_of(self, roots):
+        """the trees of ``roots``: rows of the resident trees when they hold every one of them, else built"""
+        t = self.trees
+        if t is not None and roots.shape[0]:
+            have = t.roots.cpu().numpy()
+            if have.shape[0] and np.all(have[1:] > have[:-1]):      # the resident trees' roots are ascending ids
+                idx = np.minimum(np.searchsorted(have, roots), have.shape[0] - 1)
+                if np.array_equal(have[idx], roots):
+                    return t.select(self.torch.as_tensor(idx.astype(np.int64)).to(self.device))
+        return self.construct_trees(roots)
+
+    def value_roots(self):
+        """The roots of the value line: config.value_roots of them, seeded by config.seed and fixed for the run so that
+        epochs compare.  Under torchrun, rank 0 (which evaluates) holds father-removal bits for its own root shard
+        only, so the sample comes from that shard."""
+        key = (int(config.value_roots), int(config.seed))
+        if getattr(self, "_value_key", None) != key:
+            from . import synth
+            deg = self.host_graph.degrees()
+            lo, hi = 0, self.n_node
+            if self.dist:
+                from .parallel import balanced_root_ranges
+                lo, hi = balanced_root_ranges(deg[np.asarray(self.root_nodes)] + 1, self.world)[self.rank]
+            self._value_roots = (synth.pick_roots(deg[lo:hi], key[0], seed=key[1]).astype(np.int64) + lo).astype(np.int32)
+            self._value_key = key
+        return self._value_roots
+
+    def value_line(self):
+        """The line evaluation() appends: "value:<mean V> pos:<mean pos> neg:<mean neg> roots:<ok roots>", the means taken
+        over the ok roots of value_roots() (nan when there are none)."""
+        pos, neg, ok = (x.cpu().numpy() for x in self.game_value(self.value_roots()))
+        sel = ok == 1
+        n = int(sel.sum())
+        v, p, q = ((pos + neg)[sel].mean(), pos[sel].mean(), neg[sel].mean()) if n else (np.nan,) * 3
+        return "value:%r pos:%r neg:%r roots:%d\n" % (float(v), float(p), float(q), n)
+
     def _next_tag(self):
         self.pass_counter += 1
         return self.pass_counter
@@ -290,6 +334,8 @@ class GraphGAN(object):
                     lpe = lp.LinkPredictEval(config.emb_filenames[i], config.test_filename, config.test_neg_filename,
                                              self.n_node, config.n_emb)
                 results.append(config.modes[i] + ":" + str(lpe.eval_link_prediction()) + "\n")
+        if getattr(config, "value_roots", 0) > 0:
+            results.append(self.value_line())
         os.makedirs(os.path.dirname(config.result_filename) or ".", exist_ok=True)
         with open(config.result_filename, mode="a+") as f:
             f.writelines(results)

@@ -309,13 +309,23 @@ class WalkSampler:
         ``reuse`` (default: hub_threshold > 0) scores hub lists from the per-pass cache -- the same bits either way.  The
         roots run in chunks whose scratch stays within ``max_scratch_bytes`` (default 2 GiB, env GG_GDIST_SCRATCH);
         ``counters`` (optional device int64 [16]) receives the embedding rows fetched in slot rows_gathered."""
-        torch, g = self.torch, self.g
-        assert emb.dtype == torch.float32 and emb.is_contiguous() and bias.dtype == torch.float32
-        R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
+        torch = self.torch
+        R, N = int(trees.roots.shape[0]), self.g.n_node
         dist = torch.empty((R, N), dtype=torch.float64, device=self.device)
         root_ok = torch.empty(R, dtype=torch.int32, device=self.device)
+        for _ in self._distribution_chunks(emb, bias, trees, reuse, max_scratch_bytes, counters, dist, root_ok):
+            pass
+        return dist, root_ok
+
+    def _distribution_chunks(self, emb, bias, trees, reuse, max_scratch_bytes, counters, dist=None, root_ok=None):
+        """gg_generator_dist over the roots of ``trees`` in chunks whose scratch fits the budget; yields (lo, hi, dist rows,
+        root_ok rows) per chunk.  The rows go to dist[lo:hi] / root_ok[lo:hi] when those are given, else to one chunk-sized
+        buffer that the next chunk overwrites."""
+        torch, g = self.torch, self.g
+        R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
         if R == 0:
-            return dist, root_ok
+            return
+        assert emb.dtype == torch.float32 and emb.is_contiguous() and bias.dtype == torch.float32
         reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
         budget = int(max_scratch_bytes if max_scratch_bytes is not None else os.environ.get("GG_GDIST_SCRATCH", 2 << 30))
 
@@ -325,6 +335,12 @@ class WalkSampler:
             return nb.value
         chunk = max(1, min(R, budget // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
         scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
+        if dist is None:
+            dist = torch.empty((chunk, N), dtype=torch.float64, device=self.device)
+            root_ok = torch.empty(chunk, dtype=torch.int32, device=self.device)
+            rows = lambda lo, hi: (dist[:hi - lo], root_ok[:hi - lo])
+        else:
+            rows = lambda lo, hi: (dist[lo:hi], root_ok[lo:hi])
         d = _cabi.WalkDesc()
         d.n_node, d.ld = N, int(emb.shape[1])
         d.emb, d.bias, d.indptr, d.adj = ptr(emb), ptr(bias), ptr(g.indptr), ptr(g.adj)
@@ -337,10 +353,41 @@ class WalkSampler:
             d.edge_score, d.hub_threshold = ptr(g.edge_score), self.hub_threshold
         for lo in range(0, R, chunk):
             hi = min(R, lo + chunk)
+            dr, okr = rows(lo, hi)
             d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(trees.roots[lo:hi]), ptr(trees.tree_bits[lo:hi])
-            _cabi.check(self.lib.gg_generator_dist(C.byref(d), ptr(dist[lo:hi]), ptr(root_ok[lo:hi]), ptr(scratch),
-                                                   scratch.numel(), st), "gg_generator_dist")
-        return dist, root_ok
+            _cabi.check(self.lib.gg_generator_dist(C.byref(d), ptr(dr), ptr(okr), ptr(scratch), scratch.numel(), st),
+                        "gg_generator_dist")
+            yield lo, hi, dr, okr
+
+    # ------------------------------------------------------------------ game value V(G, D)
+    def game_value(self, g_emb, g_bias, d_emb, d_bias, trees, *, max_scratch_bytes=None, reuse=None):
+        """The GraphGAN game value per root (Wang et al., AAAI-18, Eq. 1), exactly: V_c = pos_c + neg_c with
+        pos_c = E_{v ~ p_true(.|c)} log D(v, c), the mean over graph[c] (raw adjacency: duplicates and self-loops count),
+        and neg_c = E_{v ~ G(.|c)} log(1 - D(v, c)) under the generator's exact G-mode law (``distribution``, current
+        father-removal bits).  D(v, c) = sigmoid(s), s = the discriminator's fp32 score; log D = -bce(s, 1) and
+        log(1 - D) = -bce(s, 0) in fp64 (csrc/value.cu, DESIGN.md section 5.2).
+        ``g_emb, g_bias``: the generator's padded rows and bias; ``d_emb, d_bias``: the discriminator's.
+        Returns device (pos fp64 [R], neg fp64 [R], ok int32 [R]); ok = 0 (pos = neg = 0) for a root without neighbours
+        or whose G walks void.  The roots run in the chunks of ``distribution`` (same budget rule): G(. | c) exists for
+        one chunk at a time.  The bits do not depend on the chunking or on the order of the roots."""
+        torch, g = self.torch, self.g
+        assert d_emb.dtype == torch.float32 and d_emb.is_contiguous() and d_bias.dtype == torch.float32
+        assert int(d_emb.shape[0]) == g.n_node and int(d_bias.shape[0]) == g.n_node
+        R, N = int(trees.roots.shape[0]), g.n_node
+        pos = torch.zeros(R, dtype=torch.float64, device=self.device)
+        neg = torch.zeros(R, dtype=torch.float64, device=self.device)
+        ok = torch.zeros(R, dtype=torch.int32, device=self.device)
+        st, scratch = self._stream(), None
+        for lo, hi, dist, root_ok in self._distribution_chunks(g_emb, g_bias, trees, reuse, max_scratch_bytes, None):
+            nb = C.c_int64(0)
+            _cabi.check(self.lib.gg_game_value_scratch_bytes(N, hi - lo, C.byref(nb)), "gg_game_value_scratch_bytes")
+            if scratch is None or scratch.numel() < nb.value:
+                scratch = torch.empty(max(nb.value, 16), dtype=torch.uint8, device=self.device)
+            _cabi.check(self.lib.gg_game_value(N, int(d_emb.shape[1]), ptr(d_emb), ptr(d_bias), ptr(g.raw_indptr),
+                                               ptr(g.raw_adj), hi - lo, ptr(trees.roots[lo:hi]), ptr(dist), ptr(root_ok),
+                                               ptr(pos[lo:hi]), ptr(neg[lo:hi]), ptr(ok[lo:hi]), ptr(scratch),
+                                               scratch.numel(), st), "gg_game_value")
+        return pos, neg, ok
 
     def finalize(self, out):
         _cabi.check(self.lib.gg_walk_finalize(out.n_roots, ptr(out.walk_ptr), int(out.for_d), ptr(out.samples),

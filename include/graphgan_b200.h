@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 7
+#define GG_ABI_VERSION 8   /* 8: gg_game_value; 7: gg_generator_dist */
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -178,6 +178,24 @@ int gg_walk_finalize(int64_t n_roots, const int64_t *walk_ptr, int32_t for_d, in
 int gg_generator_dist_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int64_t *bytes);
 int gg_generator_dist(const gg_walk_desc *d, double *dist, int32_t *root_ok, void *scratch, int64_t scratch_bytes,
                       void *stream);
+
+/* The GraphGAN game value per root, exactly (csrc/value.cu, DESIGN.md section 5.2; Wang et al., AAAI-18, Eq. 1):
+ *   V_c = pos_c + neg_c,  pos_c = -(1 / |graph[c]|) sum_k bce(s(c, graph[c][k]), 1)  (raw CSR, entry order, duplicates and
+ *   self-loops count),  neg_c = -sum_v dist[k, v] bce(s(c, v), 0)  (v with dist[k, v] = 0 contribute exactly 0),
+ * for c = roots[k], with the discriminator's score s(c, v) = fp32 canonical dot(emb[c], emb[v]) + bias[v] (the bits of
+ * gg_pair_reward's score before its clip) and bce(s, y) = (max(s, 0) - s y) + log1p(exp(-|s|)) in fp64
+ * (sigmoid_cross_entropy_with_logits, discriminator.py:26-30).  dist / root_ok: gg_generator_dist's outputs for the same
+ * roots (the generator's G-mode law).  ok[k] = 1 iff |graph[c]| > 0 and root_ok[k] == 1; otherwise pos[k] = neg[k] = 0.
+ * Every sum runs in a fixed order: the bits depend on the inputs only, not on the number or order of the roots.
+ * emb: device [n_node, ld] (the discriminator's rows), bias: device [n_node]; raw_indptr / raw_adj: device raw CSR;
+ * roots: device [n_roots]; dist: device fp64 [n_roots, n_node]; root_ok: device [n_roots]; pos, neg: device fp64
+ * [n_roots]; ok: device [n_roots].  scratch: device, at least gg_game_value_scratch_bytes(n_node, n_roots) bytes
+ * (host-only size computation, 8 bytes per root and 512 nodes).  Two launches. */
+int gg_game_value_scratch_bytes(int64_t n_node, int64_t n_roots, int64_t *bytes);
+int gg_game_value(int64_t n_node, int32_t ld, const float *emb, const float *bias, const int64_t *raw_indptr,
+                  const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist,
+                  const int32_t *root_ok, double *pos, double *neg, int32_t *ok, void *scratch, int64_t scratch_bytes,
+                  void *stream);
 
 /* prepare_data_for_d's output rows (graph_gan.py:192-201): for every accepted root, in batch
  * order: [i]*k + [i]*k | pos + neg | 1*k + 0*k.  row_ptr: device [R+1] scratch/out (exclusive
