@@ -57,4 +57,5 @@ text_embeddings = True              # the reference's text dump (graph_gan.py:29
 binary_embeddings = False           # also dump <emb_filename>.f32 (header + [N, n_emb] fp32, row-major) every epoch
 device_eval = True                  # link-prediction check on the GPU (io/evaluation text round trip skipped)
 value_roots = 0                     # > 0: evaluation also writes "value:<V> pos:<..> neg:<..> roots:<n>", the exact game value
+value_grad = False                 # with value_roots > 0: the value line also ends in " gnorm:<|grad_G mean V|_2>", exact
                                     # (DESIGN.md section 5.2) averaged over this many seeded roots (rank 0's shard under torchrun)

@@ -16,6 +16,7 @@
 #include <math.h>
 
 #include "walk_list.cuh"
+#include "value_grad.cuh"
 
 namespace gg {
 namespace {
@@ -55,12 +56,13 @@ size_t gdist_layout(void *buf, long long n_node, long long nnz_words, long long 
     return off;
 }
 
-// One item: the law of the walk's step from node it.y of root slot it.x.
-template <int CPL>
+// One item: the law of the walk's step from node it.y of root slot it.x.  REC: also record the step law of the item's
+// list per node (DESIGN.md section 5.3): pi_in of every reached child, pi_stop of the node, the child's father.
+template <int CPL, bool REC = false>
 __device__ __forceinline__ void gdist_item(const gg_walk_desc &d, double *__restrict__ dist, int *__restrict__ root_ok,
                                            const GdView &v, const int4 it, int4 *out, unsigned *out_cnt, int *s_ids,
                                            float *s_sc, int lane, unsigned long long &rows, unsigned int (&cyc)[7],
-                                           Stage &stg) {
+                                           Stage &stg, const GdRec &rec = GdRec()) {
     const int slot = it.x, a = it.y, fa = it.z;
     const bool is_root = fa < 0, removed = it.w != 0;
     const bool inc_father = !is_root && !removed;           // graph_gan.py:250-259, G mode (d1 bits: :258-259)
@@ -117,6 +119,11 @@ __device__ __forceinline__ void gdist_item(const gg_walk_desc &d, double *__rest
         const int child = (valid && !stop) ? ids[j] : -1;
         const bool take = child >= 0 && r > 0.0;             // (a child never reached has no law below it: all zero)
         if (take) row[child] = r;
+        if constexpr (REC) {
+            const size_t o = (size_t)slot * (size_t)d.n_node;
+            if (stop) rec.pi_stop[o + a] = pi;
+            if (take) { rec.pi_in[o + child] = pi; rec.father[o + child] = a; }
+        }
         if (!is_root) warp_append(take, out, out_cnt, make_int4(slot, child, a, 0), lane);
     }
     if (!is_root) return;
@@ -173,7 +180,122 @@ gdist_kernel(const __grid_constant__ gg_walk_desc d, double *__restrict__ dist, 
     if (lane == 0 && rows && d.counters) atomicAdd(d.counters + GG_CNT_ROWS_GATHERED, rows);
 }
 
+// The same law, keeping every level: level L holds items [lev_off[L], lev_off[L + 1]) of rec.items, so that the
+// bottom-up pass of the value gradient (value_grad.cu) can replay the levels deepest first.  dist and root_ok are the bits
+// of gdist_kernel (the same item function; the item order does not enter any value).
+template <int CPL>
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, walk_min_ctas(CPL))
+gdist_rec_kernel(const __grid_constant__ gg_walk_desc d, double *__restrict__ dist, int *__restrict__ root_ok, const GdView v,
+                 const GdRec rec) {
+    extern __shared__ __align__(16) unsigned char walk_smem[];
+    cg::grid_group grid = cg::this_grid();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    float *s_sc = reinterpret_cast<float *>(walk_smem + (size_t)wid * WALK_SMEM_PER_WARP);
+    int *s_ids = reinterpret_cast<int *>(s_sc + SC_CAP);
+    Stage stg;
+    stg.buf = s_sc; stg.bar = nullptr; stg.phase = 0u; stg.on = false;
+    const long long gw = (long long)blockIdx.x * WARPS_PER_CTA + wid, nw = (long long)gridDim.x * WARPS_PER_CTA;
+    const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+    unsigned long long rows = 0;
+    unsigned int cyc[7] = {0, 0, 0, 0, 0, 0, 0};
+    for (long long k = tid; k < d.n_roots; k += nt) rec.items[k] = make_int4((int)k, __ldg(d.roots + k), -1, 0);
+    if (tid == 0) v.cnt[0] = (unsigned)d.n_roots;
+    grid.sync();
+    unsigned start = 0;                                      // first item of level lev
+    for (int lev = 0;; ++lev) {
+        const unsigned n_items = *(volatile unsigned *)(v.cnt + lev % 3);
+        if (tid == 0) rec.lev_off[lev] = start;
+        if (n_items == 0) {
+            if (tid == 0) *rec.n_lev = (unsigned)lev;
+            break;
+        }
+        if (tid == 0) v.cnt[(lev + 2) % 3] = 0;
+        const int4 *in = rec.items + start;
+        int4 *out = rec.items + start + n_items;
+        for (long long i = gw; i < (long long)n_items; i += nw)
+            gdist_item<CPL, true>(d, dist, root_ok, v, in[i], out, v.cnt + (lev + 1) % 3, s_ids, s_sc, lane, rows, cyc, stg,
+                                  rec);
+        start += n_items;
+        grid.sync();
+    }
+    for (long long k = blockIdx.x; k < d.n_roots; k += gridDim.x) {
+        if (root_ok[k] >= 0) continue;
+        double *row = dist + (size_t)k * (size_t)d.n_node;
+        for (long long i = threadIdx.x; i < d.n_node; i += blockDim.x) row[i] = 0.0;
+        __syncthreads();
+        if (threadIdx.x == 0) root_ok[k] = 0;
+    }
+    if (lane == 0 && rows && d.counters) atomicAdd(d.counters + GG_CNT_ROWS_GATHERED, rows);
+}
+
+// cooperative launch of `kern` (gdist_kernel / gdist_rec_kernel) over the whole device
+int launch_gdist(const void *kern, const gg_walk_desc &d, void **args, cudaStream_t st) {
+    int dev = 0, coop = 0;
+    GG_CHECK(cudaGetDevice(&dev));
+    GG_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+    GG_REQUIRE(coop, "device does not support cooperative launches");
+    const int cpl = d.ld / 32, nt = WARPS_PER_CTA * 32;
+    const int smem = walk_smem_bytes(cpl, WARPS_PER_CTA);
+    GG_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    int per_sm = 0;
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, nt, smem));
+    GG_REQUIRE(per_sm >= 1, "generator distribution kernel does not fit on an SM");
+    if (per_sm > walk_min_ctas(cpl)) per_sm = walk_min_ctas(cpl);
+    GG_CHECK(cudaLaunchCooperativeKernel(kern, dim3((unsigned)(sm_count() * per_sm)), dim3(nt), args, (size_t)smem, st));
+    return 0;
+}
+
+// the recording variant's scratch: counters, every level's items and their offsets, the list pools of gdist_layout
+size_t rec_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, GdRec *rec, GdView *v) {
+    const long long stride = 32 * nnz_words + n_node;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t o_cnt = take(3 * sizeof(unsigned));
+    const size_t o_items = take((size_t)n_roots * (size_t)n_node * sizeof(int4));
+    const size_t o_lev = take(((size_t)n_node + 2) * sizeof(unsigned));
+    const size_t o_nlev = take(sizeof(unsigned));
+    const size_t o_ids = take((size_t)n_roots * (size_t)stride * sizeof(int));
+    const size_t o_sc = take((size_t)n_roots * (size_t)stride * sizeof(float));
+    unsigned char *b = static_cast<unsigned char *>(buf);
+    if (b && rec) {
+        rec->items = reinterpret_cast<int4 *>(b + o_items);
+        rec->lev_off = reinterpret_cast<unsigned *>(b + o_lev);
+        rec->n_lev = reinterpret_cast<unsigned *>(b + o_nlev);
+    }
+    if (b && v) {
+        v->cnt = reinterpret_cast<unsigned *>(b + o_cnt);
+        v->list[0] = v->list[1] = nullptr;
+        v->pool_ids = reinterpret_cast<int *>(b + o_ids);
+        v->pool_sc = reinterpret_cast<float *>(b + o_sc);
+        v->pool_stride = stride;
+    }
+    return off;
+}
+
 }  // namespace
+
+size_t gdist_rec_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, GdRec *rec) {
+    return rec_layout(buf, n_node, nnz_words, n_roots, rec, nullptr);
+}
+
+int gdist_rec_launch(const gg_walk_desc &d, double *dist, int *root_ok, GdRec rec, void *scratch, cudaStream_t st) {
+    GdView v;
+    rec_layout(scratch, d.n_node, d.tree_words - 1, d.n_roots, &rec, &v);
+    GG_CHECK(cudaMemsetAsync(v.cnt, 0, 3 * sizeof(unsigned), st));
+    const void *kern;
+    switch (d.ld / 32) {
+        case 1: kern = (const void *)gdist_rec_kernel<1>; break;
+        case 2: kern = (const void *)gdist_rec_kernel<2>; break;
+        case 4: kern = (const void *)gdist_rec_kernel<4>; break;
+        case 8: kern = (const void *)gdist_rec_kernel<8>; break;
+        default: kern = (const void *)gdist_rec_kernel<16>; break;
+    }
+    double *dist_p = dist;
+    int *ok_p = root_ok;
+    void *args[] = {(void *)&d, (void *)&dist_p, (void *)&ok_p, (void *)&v, (void *)&rec};
+    return launch_gdist(kern, d, args, st);
+}
+
 }  // namespace gg
 
 extern "C" int gg_generator_dist_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int64_t *bytes) {
@@ -200,10 +322,6 @@ extern "C" int gg_generator_dist(const gg_walk_desc *dp, double *dist, int32_t *
     GG_CHECK(cudaMemsetAsync(dist, 0, sizeof(double) * (size_t)d.n_roots * (size_t)d.n_node, st));
     GG_CHECK(cudaMemsetAsync(root_ok, 0, sizeof(int32_t) * (size_t)d.n_roots, st));
     GG_CHECK(cudaMemsetAsync(v.cnt, 0, 3 * sizeof(unsigned), st));
-    int dev = 0, coop = 0;
-    GG_CHECK(cudaGetDevice(&dev));
-    GG_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-    GG_REQUIRE(coop, "device does not support cooperative launches");
     const void *kern;
     switch (d.ld / 32) {
         case 1: kern = (const void *)gg::gdist_kernel<1>; break;
@@ -213,16 +331,8 @@ extern "C" int gg_generator_dist(const gg_walk_desc *dp, double *dist, int32_t *
         case 16: kern = (const void *)gg::gdist_kernel<16>; break;
         default: gg::set_error("gg_generator_dist: unsupported ld %d (supported: 32, 64, 128, 256, 512)", d.ld); return 2;
     }
-    const int cpl = d.ld / 32, nt = gg::WARPS_PER_CTA * 32;
-    const int smem = gg::walk_smem_bytes(cpl, gg::WARPS_PER_CTA);
-    GG_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, nt, smem));
-    GG_REQUIRE(per_sm >= 1, "generator distribution kernel does not fit on an SM");
-    if (per_sm > gg::walk_min_ctas(cpl)) per_sm = gg::walk_min_ctas(cpl);
     double *dist_p = dist;
     int *ok_p = root_ok;
     void *args[] = {(void *)&d, (void *)&dist_p, (void *)&ok_p, (void *)&v};
-    GG_CHECK(cudaLaunchCooperativeKernel(kern, dim3((unsigned)(gg::sm_count() * per_sm)), dim3(nt), args, (size_t)smem, st));
-    return 0;
+    return gg::launch_gdist(kern, d, args, st);
 }

@@ -17,6 +17,7 @@
 #include <math.h>
 
 #include "gg_common.cuh"
+#include "value_grad.cuh"
 
 namespace gg {
 namespace {
@@ -119,9 +120,10 @@ __device__ void pos_item(const ValArgs &a, long long k, double *s_part) {
     __syncthreads();
 }
 
-// The tile partials of neg for root tile rt (roots rt * RT ..) and node tile t; the root rows are in s_root.
-template <int CPL>
-__device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_root, double *s_part) {
+// The tile partials of neg for root tile rt (roots rt * RT ..) and node tile t; the root rows are in s_root.  STORE: each
+// product h[k, v] = dist[k, v] * bce(s(c_k, v), 0) is stored instead of added (the value gradient, DESIGN.md section 5.3).
+template <int CPL, bool STORE = false>
+__device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_root, double *s_part, double *h = nullptr) {
     constexpr int LD = 32 * CPL, RT = val_root_tile(CPL), RJ = RT / 8;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane & 7, grp = threadIdx.x >> 3;
     const long long k0 = (long long)rt * RT;
@@ -154,21 +156,29 @@ __device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_r
                 s[r] = x;
             }
             const float sc = __fadd_rn(group8_sum8(s, g), bv);
-            if (w[j] != 0.0) acc[j] = __dadd_rn(acc[j], __dmul_rn(w[j], bce_logits(sc, false)));
+            if constexpr (STORE) {
+                const long long k = k0 + 8 * j + g;
+                if (valid && k < a.n_roots)
+                    h[(size_t)k * (size_t)a.n_node + (size_t)v] = (w[j] != 0.0) ? __dmul_rn(w[j], bce_logits(sc, false)) : 0.0;
+            } else {
+                if (w[j] != 0.0) acc[j] = __dadd_rn(acc[j], __dmul_rn(w[j], bce_logits(sc, false)));
+            }
         }
     }
+    if constexpr (!STORE) {
 #pragma unroll
-    for (int j = 0; j < RJ; ++j) {
-        const double x = warp_groups_sum(acc[j]);
-        if (lane < 8) s_part[wid * RT + 8 * j + lane] = x;
+        for (int j = 0; j < RJ; ++j) {
+            const double x = warp_groups_sum(acc[j]);
+            if (lane < 8) s_part[wid * RT + 8 * j + lane] = x;
+        }
+        __syncthreads();
+        if (threadIdx.x < RT && k0 + threadIdx.x < a.n_roots) {
+            double x = s_part[threadIdx.x];
+            for (int w = 1; w < VAL_THREADS / 32; ++w) x = __dadd_rn(x, s_part[w * RT + threadIdx.x]);
+            a.partial[(size_t)(k0 + threadIdx.x) * (size_t)a.n_tiles + (size_t)t] = x;
+        }
+        __syncthreads();
     }
-    __syncthreads();
-    if (threadIdx.x < RT && k0 + threadIdx.x < a.n_roots) {
-        double x = s_part[threadIdx.x];
-        for (int w = 1; w < VAL_THREADS / 32; ++w) x = __dadd_rn(x, s_part[w * RT + threadIdx.x]);
-        a.partial[(size_t)(k0 + threadIdx.x) * (size_t)a.n_tiles + (size_t)t] = x;
-    }
-    __syncthreads();
 }
 
 // Work items: first one pos item per root (a hub root's list is the longest single item, so it starts first), then the
@@ -199,6 +209,32 @@ __global__ void __launch_bounds__(VAL_THREADS) value_kernel(const ValArgs a) {
             cur_rt = rt;
         }
         neg_item<CPL>(a, (int)rt, t, s_root, s_part);
+    }
+}
+
+// h[k, v] for every (root, node) pair: value_kernel's neg items with a store instead of the chain
+template <int CPL>
+__global__ void __launch_bounds__(VAL_THREADS) value_h_kernel(const ValArgs a, double *__restrict__ h) {
+    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
+    extern __shared__ __align__(16) unsigned char val_smem[];
+    float *s_root = reinterpret_cast<float *>(val_smem);
+    double *s_part = reinterpret_cast<double *>(val_smem + (size_t)RT * LD * sizeof(float));
+    const long long n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
+    long long cur_rt = -1;
+    for (long long item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const long long rt = item / a.n_tiles, t = item % a.n_tiles;
+        if (rt != cur_rt) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
+                const long long k = rt * RT + i / (LD / 4);
+                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
+                reinterpret_cast<float4 *>(s_root)[i] = x;
+            }
+            __syncthreads();
+            cur_rt = rt;
+        }
+        neg_item<CPL, true>(a, (int)rt, t, s_root, s_part, h);
     }
 }
 
@@ -236,7 +272,36 @@ int launch_value(const ValArgs &a, double *neg, int *ok, cudaStream_t st) {
     return check_cuda(cudaGetLastError(), "game value reduce launch");
 }
 
+template <int CPL>
+int launch_value_h(const ValArgs &a, double *h, cudaStream_t st) {
+    const size_t smem = val_smem_bytes(CPL);
+    int per_sm = 0;
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_h_kernel<CPL>, VAL_THREADS, smem));
+    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
+    const long long RT = val_root_tile(CPL), n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
+    long long grid = (long long)sm_count() * per_sm;
+    if (grid > n_items) grid = n_items;
+    value_h_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a, h);
+    return check_cuda(cudaGetLastError(), "game value h launch");
+}
+
 }  // namespace
+
+int value_h_launch(long long n_node, int ld, const float *emb, const float *bias, long long n_roots, const int *roots,
+                   const double *dist, double *h, cudaStream_t st) {
+    if (n_roots == 0) return 0;
+    ValArgs a = {};
+    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = val_tiles(n_node);
+    a.emb = emb; a.bias = bias; a.roots = roots; a.dist = dist;
+    switch (ld / 32) {
+        case 1: return launch_value_h<1>(a, h, st);
+        case 2: return launch_value_h<2>(a, h, st);
+        case 4: return launch_value_h<4>(a, h, st);
+        case 8: return launch_value_h<8>(a, h, st);
+        default: return launch_value_h<16>(a, h, st);
+    }
+}
+
 }  // namespace gg
 
 extern "C" int gg_game_value_scratch_bytes(int64_t n_node, int64_t n_roots, int64_t *bytes) {

@@ -137,6 +137,14 @@ class GraphGAN(object):
         g, d = self.generator, self.discriminator
         return self.sampler.game_value(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
 
+    def game_value_grad(self, roots):
+        """game_value(roots) and the exact gradient of sum_{ok c} V_c with respect to the generator's padded rows and biases
+        (DESIGN.md section 5.3): sampler.WalkSampler.game_value_grad.  Returns device (pos, neg, ok, grad_emb fp64 [N, ld],
+        grad_bias fp64 [N]); pos, neg and ok are the bits of game_value."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        return self.sampler.game_value_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
+
     def _trees_of(self, roots):
         """the trees of ``roots``: rows of the resident trees when they hold every one of them, else built"""
         t = self.trees
@@ -166,12 +174,21 @@ class GraphGAN(object):
 
     def value_line(self):
         """The line evaluation() appends: "value:<mean V> pos:<mean pos> neg:<mean neg> roots:<ok roots>", the means taken
-        over the ok roots of value_roots() (nan when there are none)."""
-        pos, neg, ok = (x.cpu().numpy() for x in self.game_value(self.value_roots()))
+        over the ok roots of value_roots() (nan when there are none).  With config.value_grad, " gnorm:<norm>" follows:
+        the 2-norm of the gradient of the mean V over (E_G[:, :n_emb], b_G), exact (game_value_grad)."""
+        if getattr(config, "value_grad", False):
+            pos, neg, ok, g_emb, g_bias = self.game_value_grad(self.value_roots())
+        else:
+            pos, neg, ok = self.game_value(self.value_roots())
+        pos, neg, ok = (x.cpu().numpy() for x in (pos, neg, ok))
         sel = ok == 1
         n = int(sel.sum())
         v, p, q = ((pos + neg)[sel].mean(), pos[sel].mean(), neg[sel].mean()) if n else (np.nan,) * 3
-        return "value:%r pos:%r neg:%r roots:%d\n" % (float(v), float(p), float(q), n)
+        line = "value:%r pos:%r neg:%r roots:%d" % (float(v), float(p), float(q), n)
+        if getattr(config, "value_grad", False):
+            sq = float((g_emb[:, :self.generator.n_emb] ** 2).sum().item() + (g_bias ** 2).sum().item())
+            line += " gnorm:%r" % (float(np.sqrt(sq) / n) if n else np.nan)
+        return line + "\n"
 
     def _next_tag(self):
         self.pass_counter += 1

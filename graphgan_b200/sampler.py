@@ -317,6 +317,21 @@ class WalkSampler:
             pass
         return dist, root_ok
 
+    def _law_desc(self, emb, bias, trees, reuse, counters):
+        """the descriptor of the generator's law for gg_generator_dist / gg_game_value_grad (the per-chunk fields n_roots,
+        roots, tree_bits are the caller's); with ``reuse``, the hub scores are refreshed first"""
+        g = self.g
+        d = _cabi.WalkDesc()
+        d.n_node, d.ld = g.n_node, int(emb.shape[1])
+        d.emb, d.bias, d.indptr, d.adj = ptr(emb), ptr(bias), ptr(g.indptr), ptr(g.adj)
+        d.tree_words, d.d1_bits, d.counters = int(trees.tree_bits.shape[1]), ptr(g.d1_bits), ptr(counters)
+        if reuse:
+            items, pairs, n_items, _ = g.hub_tiles(self.hub_threshold)
+            _cabi.check(self.lib.gg_hub_scores(n_items, ptr(items), ptr(pairs), ptr(emb), ptr(bias), int(emb.shape[1]),
+                                               ptr(g.edge_score), self._stream()), "gg_hub_scores")
+            d.edge_score, d.hub_threshold = ptr(g.edge_score), self.hub_threshold
+        return d
+
     def _distribution_chunks(self, emb, bias, trees, reuse, max_scratch_bytes, counters, dist=None, root_ok=None):
         """gg_generator_dist over the roots of ``trees`` in chunks whose scratch fits the budget; yields (lo, hi, dist rows,
         root_ok rows) per chunk.  The rows go to dist[lo:hi] / root_ok[lo:hi] when those are given, else to one chunk-sized
@@ -341,16 +356,8 @@ class WalkSampler:
             rows = lambda lo, hi: (dist[:hi - lo], root_ok[:hi - lo])
         else:
             rows = lambda lo, hi: (dist[lo:hi], root_ok[lo:hi])
-        d = _cabi.WalkDesc()
-        d.n_node, d.ld = N, int(emb.shape[1])
-        d.emb, d.bias, d.indptr, d.adj = ptr(emb), ptr(bias), ptr(g.indptr), ptr(g.adj)
-        d.tree_words, d.d1_bits, d.counters = int(trees.tree_bits.shape[1]), ptr(g.d1_bits), ptr(counters)
+        d = self._law_desc(emb, bias, trees, reuse, counters)
         st = self._stream()
-        if reuse:
-            items, pairs, n_items, _ = g.hub_tiles(self.hub_threshold)
-            _cabi.check(self.lib.gg_hub_scores(n_items, ptr(items), ptr(pairs), ptr(emb), ptr(bias), int(emb.shape[1]),
-                                               ptr(g.edge_score), st), "gg_hub_scores")
-            d.edge_score, d.hub_threshold = ptr(g.edge_score), self.hub_threshold
         for lo in range(0, R, chunk):
             hi = min(R, lo + chunk)
             dr, okr = rows(lo, hi)
@@ -388,6 +395,51 @@ class WalkSampler:
                                                ptr(pos[lo:hi]), ptr(neg[lo:hi]), ptr(ok[lo:hi]), ptr(scratch),
                                                scratch.numel(), st), "gg_game_value")
         return pos, neg, ok
+
+    # ------------------------------------------------------------------ generator gradient of V(G, D)
+    def game_value_grad(self, g_emb, g_bias, d_emb, d_bias, trees, *, max_scratch_bytes=None, reuse=None):
+        """``game_value`` and the exact gradient of sum_{ok c} V_c with respect to the generator's parameters (csrc/
+        value_grad.cu, DESIGN.md section 5.3): the policy gradient sum_v G(v | c) grad log G(v | c) log(1 - D(v, c)) of
+        the paper, evaluated exactly over the BFS trees under the step law of ``distribution``.
+        Returns device (pos fp64 [R], neg fp64 [R], ok int32 [R]) in the order of ``trees`` -- the bits of ``game_value``
+        -- and (grad_emb fp64 [N, ld], grad_bias fp64 [N]) for the padded rows ``g_emb`` (pad columns exactly 0) and
+        ``g_bias``.  The roots are taken in ascending id order (stable for duplicates), in chunks under the budget rule of
+        ``distribution`` (``max_scratch_bytes``, default 2 GiB or env GG_GDIST_SCRATCH), each coordinate one fp64 chain
+        over the roots: the bits do not depend on the chunking, the order of the roots or the call."""
+        torch, g = self.torch, self.g
+        assert g_emb.dtype == torch.float32 and g_emb.is_contiguous() and g_bias.dtype == torch.float32
+        assert d_emb.dtype == torch.float32 and d_emb.is_contiguous() and d_bias.dtype == torch.float32
+        assert d_emb.shape == g_emb.shape and int(d_bias.shape[0]) == g.n_node and int(g_emb.shape[0]) == g.n_node
+        R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
+        pos = torch.zeros(R, dtype=torch.float64, device=self.device)
+        neg = torch.zeros(R, dtype=torch.float64, device=self.device)
+        ok = torch.zeros(R, dtype=torch.int32, device=self.device)
+        grad_emb = torch.zeros(tuple(g_emb.shape), dtype=torch.float64, device=self.device)
+        grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
+        if R == 0:
+            return pos, neg, ok, grad_emb, grad_bias
+        order = torch.argsort(trees.roots.long(), stable=True)
+        st_trees = trees.select(order)
+        reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
+        budget = int(max_scratch_bytes if max_scratch_bytes is not None else os.environ.get("GG_GDIST_SCRATCH", 2 << 30))
+
+        def scratch_bytes(k):
+            nb = C.c_int64(0)
+            _cabi.check(self.lib.gg_game_value_grad_scratch_bytes(N, nnz, k, C.byref(nb)), "gg_game_value_grad_scratch_bytes")
+            return nb.value
+        chunk = max(1, min(R, budget // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
+        sp, sn, so = (torch.zeros_like(x) for x in (pos, neg, ok))
+        d = self._law_desc(g_emb, g_bias, st_trees, reuse, None)
+        st = self._stream()
+        for lo in range(0, R, chunk):
+            hi = min(R, lo + chunk)
+            d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(st_trees.roots[lo:hi]), ptr(st_trees.tree_bits[lo:hi])
+            _cabi.check(self.lib.gg_game_value_grad(C.byref(d), ptr(d_emb), ptr(d_bias), ptr(g.raw_indptr), ptr(g.raw_adj),
+                                                    ptr(sp[lo:hi]), ptr(sn[lo:hi]), ptr(so[lo:hi]), ptr(grad_emb),
+                                                    ptr(grad_bias), ptr(scratch), scratch.numel(), st), "gg_game_value_grad")
+        pos[order], neg[order], ok[order] = sp, sn, so
+        return pos, neg, ok, grad_emb, grad_bias
 
     def finalize(self, out):
         _cabi.check(self.lib.gg_walk_finalize(out.n_roots, ptr(out.walk_ptr), int(out.for_d), ptr(out.samples),

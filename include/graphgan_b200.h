@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 8   /* 8: gg_game_value; 7: gg_generator_dist */
+#define GG_ABI_VERSION 9   /* 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -196,6 +196,22 @@ int gg_game_value(int64_t n_node, int32_t ld, const float *emb, const float *bia
                   const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist,
                   const int32_t *root_ok, double *pos, double *neg, int32_t *ok, void *scratch, int64_t scratch_bytes,
                   void *stream);
+
+/* The exact generator gradient of the game value (csrc/value_grad.cu, DESIGN.md section 5.3): for the roots of g (the
+ * generator's law as gg_generator_dist computes it from g's fields) and the discriminator d_emb / d_bias, writes pos, neg
+ * and ok with the bits of gg_game_value and ADDS the gradient of sum_{ok c} V_c with respect to the generator's padded rows
+ * (g->emb, ld columns) and biases into grad_emb (device fp64 [n_node, ld]) and grad_bias (device fp64 [n_node]):
+ *   grad_G V_c = -sum over lists a, candidates x of w_a(x) grad s(a, x),  w_a(x) = F_a(x) - pi_a(x) T(a),
+ * T(a) = the sum of h(u) = G(u | c) bce(s_D(c, u), 0) over the subtree of a, F_a(x) = T(x) for a child, h(a) for the father.
+ * Pad columns receive exactly 0.  Each node's row takes the roots in the order given as one fp64 chain per coordinate,
+ * continued from the value already in grad_emb / grad_bias: pass the roots in ascending id order (and chunks in order)
+ * for bits that do not depend on the order or the chunking.  d_emb has g->ld columns.  Other arguments as for
+ * gg_generator_dist and gg_game_value.  scratch: device, at least gg_game_value_grad_scratch_bytes(n_node, nnz, n_roots)
+ * bytes (host-only size computation; gg_generator_dist's plus 28 bytes per (root, node)). */
+int gg_game_value_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int64_t *bytes);
+int gg_game_value_grad(const gg_walk_desc *g, const float *d_emb, const float *d_bias, const int64_t *raw_indptr,
+                       const int32_t *raw_adj, double *pos, double *neg, int32_t *ok, double *grad_emb, double *grad_bias,
+                       void *scratch, int64_t scratch_bytes, void *stream);
 
 /* prepare_data_for_d's output rows (graph_gan.py:192-201): for every accepted root, in batch
  * order: [i]*k + [i]*k | pos + neg | 1*k + 0*k.  row_ptr: device [R+1] scratch/out (exclusive
