@@ -8,7 +8,8 @@
 //   gg_pair_dot_f64  : float64 dot of two embedding rows per test edge (the text round trip of an fp32 value is exact,
 //                      so these are the reference's operands; products of fp32 values are exact in fp64)
 //   gg_link_pred_acc : np.median (mean of the two middle order statistics for even counts) by an MSB-first radix
-//                      select over order-preserving 64-bit keys, then the accuracy count -- one CTA, no sort
+//                      select over order-preserving 64-bit keys, then the accuracy count -- one CTA, no sort; a NaN
+//                      score gives np.median's NaN (and so no positive prediction), as the reference reports it
 //   gg_unpad_rows    : [N, ld] padded rows -> dense [N, n_emb] fp32, the binary dump's payload
 // Gather-bound / tiny; no tensor cores.
 #include "gg_common.cuh"
@@ -84,22 +85,29 @@ __global__ void __launch_bounds__(1024, 1) link_pred_kernel(long long n, const d
     __shared__ unsigned hist[256];
     __shared__ unsigned long long s_prefix;
     __shared__ long long s_k;
-    __shared__ unsigned long long s_hits;
+    __shared__ unsigned long long s_hits, s_nans;
     // np.median: middle element (odd n) or the mean of the two middle elements (even n)
     const double hi = key_value(radix_select(score, n, n / 2, hist, &s_prefix, &s_k));
     const double lo = (n % 2) ? hi : key_value(radix_select(score, n, n / 2 - 1, hist, &s_prefix, &s_k));
     const double med = (n % 2) ? hi : (lo + hi) / 2.0;
-    if (threadIdx.x == 0) s_hits = 0ull;
+    if (threadIdx.x == 0) { s_hits = 0ull; s_nans = 0ull; }
     __syncthreads();
     const long long half = n / 2;                 // true_label[0 : len // 2] = 1 (link_prediction.py:34-35)
-    unsigned long long hits = 0;
+    unsigned long long hits = 0, nans = 0;
     for (long long i = threadIdx.x; i < n; i += blockDim.x) {
-        const bool pred = score[i] >= med;        // index_pos = test_label >= median (:30)
+        const double x = score[i];
+        const bool pred = x >= med;               // index_pos = test_label >= median (:30)
         hits += (pred == (i < half)) ? 1ull : 0ull;
+        nans += isnan(x) ? 1ull : 0ull;
     }
     atomicAdd(&s_hits, hits);
+    atomicAdd(&s_nans, nans);
     __syncthreads();
-    if (threadIdx.x == 0) { out[0] = (double)s_hits / (double)n; out[1] = med; }
+    // any NaN makes np.median NaN (order_key sorts NaN to an end instead), so no score is >= it: every prediction is 0
+    if (threadIdx.x == 0) {
+        out[0] = s_nans ? (double)(n - half) / (double)n : (double)s_hits / (double)n;
+        out[1] = s_nans ? __longlong_as_double(0x7ff8000000000000ll) : med;
+    }
 }
 
 __global__ void unpad_rows_kernel(long long n_node, int ld, int d, const float *__restrict__ emb, float *__restrict__ out) {

@@ -431,7 +431,8 @@ int gg_train_fused(int32_t mode, int64_t n_rows, const int64_t *start_list_dev, 
  * LinkPredictEval.eval_link_prediction (src/evaluation/link_prediction.py:19-38).
  *   gg_pair_dot_f64  : out[k] = float64 dot of rows node_id[k], node_neighbor_id[k] (np.dot on the re-read rows)
  *   gg_link_pred_acc : out2[0] = accuracy of (score >= np.median(score)) against labels [1]*(n/2) + [0]*(n - n/2),
- *                      out2[1] = the median; score / out2: device float64
+ *                      out2[1] = the median; score / out2: device float64.  Any NaN score makes the median NaN and
+ *                      the accuracy (n - n/2) / n, as np.median and the >= comparison give them
  *   gg_unpad_rows    : dense [N, n_emb] fp32 copy of the padded [N, ld] rows (payload of the binary dump)
  * ------------------------------------------------------------------------------------------ */
 int gg_pair_dot_f64(int64_t n_pairs, const int32_t *node_id, const int32_t *node_neighbor_id, const float *emb,
