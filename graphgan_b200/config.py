@@ -59,3 +59,4 @@ device_eval = True                  # link-prediction check on the GPU (io/evalu
 value_roots = 0                     # > 0: evaluation also writes "value:<V> pos:<..> neg:<..> roots:<n>", the exact game value
 value_grad = False                 # with value_roots > 0: the value line also ends in " gnorm:<|grad_G mean V|_2>", exact
                                     # (DESIGN.md section 5.2) averaged over this many seeded roots (rank 0's shard under torchrun)
+value_grad_d = False               # with value_roots > 0: the value line ends in " dnorm:<|grad_D mean V|_2>", exact (section 5.4)

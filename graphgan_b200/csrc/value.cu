@@ -120,16 +120,41 @@ __device__ void pos_item(const ValArgs &a, long long k, double *s_part) {
     __syncthreads();
 }
 
-// The tile partials of neg for root tile rt (roots rt * RT ..) and node tile t; the root rows are in s_root.  STORE: each
+// dV_c / ds(c, v) = m sigma(-s) / deg_c - G sigma(s) (DESIGN.md section 5.4): m the multiplicity of v in graph[c], G the
+// law's dist[k, v]; sigma(|s|) = 1 / (1 + e), sigma(-|s|) = e sigma(|s|), e = exp(-|s|), in fp64 from the fp32 s
+__device__ __forceinline__ double dgrad_w(int m, double deg, double G, float s) {
+    if (m == 0 && G == 0.0) return 0.0;
+    const double x = (double)s, e = exp(-fabs(x));
+    const double big = __drcp_rn(__dadd_rn(1.0, e)), small = __dmul_rn(e, big);
+    const double sp = x >= 0.0 ? big : small, sn = x >= 0.0 ? small : big;
+    const double pos = m != 0 ? __ddiv_rn(__dmul_rn((double)m, sn), deg) : 0.0;
+    return __dsub_rn(pos, G != 0.0 ? __dmul_rn(G, sp) : 0.0);
+}
+
+enum class NegOut { Chain, H, W };
+
+// The tile partials of neg for root tile rt (roots rt * RT ..) and node tile t; the root rows are in s_root.  OUT = H: each
 // product h[k, v] = dist[k, v] * bce(s(c_k, v), 0) is stored instead of added (the value gradient, DESIGN.md section 5.3).
-template <int CPL, bool STORE = false>
-__device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_root, double *s_part, double *h = nullptr) {
+// OUT = W: h[k, v] = dgrad_w of the multiplicity mult[k, v] and dist[k, v] is stored, 0 for roots with ok_k = 0 (the
+// discriminator gradient, section 5.4).
+template <int CPL, NegOut OUT = NegOut::Chain>
+__device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_root, double *s_part, double *h = nullptr,
+                         const int *mult = nullptr) {
     constexpr int LD = 32 * CPL, RT = val_root_tile(CPL), RJ = RT / 8;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane & 7, grp = threadIdx.x >> 3;
     const long long k0 = (long long)rt * RT;
     double acc[RJ];
 #pragma unroll
     for (int j = 0; j < RJ; ++j) acc[j] = 0.0;
+    double rdeg[OUT == NegOut::W ? RJ : 1];           // W: |graph[c_k]| of lane g's roots, 0 when ok_k = 0
+    if constexpr (OUT == NegOut::W) {
+#pragma unroll
+        for (int j = 0; j < RJ; ++j) {
+            const long long k = k0 + 8 * j + g;
+            long long lo, deg;
+            rdeg[j] = (k < a.n_roots && value_ok(a, k, lo, deg)) ? (double)deg : 0.0;
+        }
+    }
     for (int i = 0; i < VAL_NPG; ++i) {
         const long long v = t * VAL_TILE + grp + (long long)VAL_GROUPS * i;
         const bool valid = v < a.n_node;
@@ -156,16 +181,22 @@ __device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_r
                 s[r] = x;
             }
             const float sc = __fadd_rn(group8_sum8(s, g), bv);
-            if constexpr (STORE) {
+            if constexpr (OUT == NegOut::H) {
                 const long long k = k0 + 8 * j + g;
                 if (valid && k < a.n_roots)
                     h[(size_t)k * (size_t)a.n_node + (size_t)v] = (w[j] != 0.0) ? __dmul_rn(w[j], bce_logits(sc, false)) : 0.0;
+            } else if constexpr (OUT == NegOut::W) {
+                const long long k = k0 + 8 * j + g;
+                if (valid && k < a.n_roots) {
+                    const size_t o = (size_t)k * (size_t)a.n_node + (size_t)v;
+                    h[o] = rdeg[j] > 0.0 ? dgrad_w(__ldg(mult + o), rdeg[j], w[j], sc) : 0.0;
+                }
             } else {
                 if (w[j] != 0.0) acc[j] = __dadd_rn(acc[j], __dmul_rn(w[j], bce_logits(sc, false)));
             }
         }
     }
-    if constexpr (!STORE) {
+    if constexpr (OUT == NegOut::Chain) {
 #pragma unroll
         for (int j = 0; j < RJ; ++j) {
             const double x = warp_groups_sum(acc[j]);
@@ -234,7 +265,34 @@ __global__ void __launch_bounds__(VAL_THREADS) value_h_kernel(const ValArgs a, d
             __syncthreads();
             cur_rt = rt;
         }
-        neg_item<CPL, true>(a, (int)rt, t, s_root, s_part, h);
+        neg_item<CPL, NegOut::H>(a, (int)rt, t, s_root, s_part, h);
+    }
+}
+
+// W[k, v] = dV_{c_k} / ds(c_k, v) for every (root, node) pair: value_kernel's neg items with a store of dgrad_w
+template <int CPL>
+__global__ void __launch_bounds__(VAL_THREADS) value_w_kernel(const ValArgs a, const int *__restrict__ mult,
+                                                              double *__restrict__ W) {
+    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
+    extern __shared__ __align__(16) unsigned char val_smem[];
+    float *s_root = reinterpret_cast<float *>(val_smem);
+    double *s_part = reinterpret_cast<double *>(val_smem + (size_t)RT * LD * sizeof(float));
+    const long long n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
+    long long cur_rt = -1;
+    for (long long item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const long long rt = item / a.n_tiles, t = item % a.n_tiles;
+        if (rt != cur_rt) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
+                const long long k = rt * RT + i / (LD / 4);
+                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
+                reinterpret_cast<float4 *>(s_root)[i] = x;
+            }
+            __syncthreads();
+            cur_rt = rt;
+        }
+        neg_item<CPL, NegOut::W>(a, (int)rt, t, s_root, s_part, W, mult);
     }
 }
 
@@ -285,7 +343,36 @@ int launch_value_h(const ValArgs &a, double *h, cudaStream_t st) {
     return check_cuda(cudaGetLastError(), "game value h launch");
 }
 
+template <int CPL>
+int launch_value_w(const ValArgs &a, const int *mult, double *W, cudaStream_t st) {
+    const size_t smem = val_smem_bytes(CPL);
+    int per_sm = 0;
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_w_kernel<CPL>, VAL_THREADS, smem));
+    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
+    const long long RT = val_root_tile(CPL), n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
+    long long grid = (long long)sm_count() * per_sm;
+    if (grid > n_items) grid = n_items;
+    value_w_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a, mult, W);
+    return check_cuda(cudaGetLastError(), "game value W launch");
+}
+
 }  // namespace
+
+int value_w_launch(long long n_node, int ld, const float *emb, const float *bias, const long long *raw_indptr,
+                   long long n_roots, const int *roots, const double *dist, const int *root_ok, const int *mult, double *W,
+                   cudaStream_t st) {
+    if (n_roots == 0) return 0;
+    ValArgs a = {};
+    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = val_tiles(n_node);
+    a.emb = emb; a.bias = bias; a.raw_indptr = raw_indptr; a.roots = roots; a.dist = dist; a.root_ok = root_ok;
+    switch (ld / 32) {
+        case 1: return launch_value_w<1>(a, mult, W, st);
+        case 2: return launch_value_w<2>(a, mult, W, st);
+        case 4: return launch_value_w<4>(a, mult, W, st);
+        case 8: return launch_value_w<8>(a, mult, W, st);
+        default: return launch_value_w<16>(a, mult, W, st);
+    }
+}
 
 int value_h_launch(long long n_node, int ld, const float *emb, const float *bias, long long n_roots, const int *roots,
                    const double *dist, double *h, cudaStream_t st) {

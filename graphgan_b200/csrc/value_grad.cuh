@@ -1,5 +1,5 @@
-// value_grad.cuh -- what the exact generator gradient of the game value (value_grad.cu, DESIGN.md section 5.3) takes from
-// the generator distribution (gdist.cu) and the game value (value.cu).
+// value_grad.cuh -- what the exact gradients of the game value (value_grad.cu and value_dgrad.cu, DESIGN.md sections 5.3
+// and 5.4) take from the generator distribution (gdist.cu) and the game value (value.cu).
 #pragma once
 #include "gg_common.cuh"
 
@@ -23,5 +23,10 @@ int gdist_rec_launch(const gg_walk_desc &d, double *dist, int *root_ok, GdRec re
 // h[k, v] = dist[k, v] * bce(s(roots[k], v), 0) (0 where dist is 0): the products the value kernel adds into neg
 int value_h_launch(long long n_node, int ld, const float *emb, const float *bias, long long n_roots, const int *roots,
                    const double *dist, double *h, cudaStream_t st);
+// W[k, v] = dV_{c_k} / ds(c_k, v) = mult[k, v] sigma(-s) / |graph[c_k]| - dist[k, v] sigma(s), 0 for roots with ok_k = 0
+// (the discriminator gradient, value_dgrad.cu, DESIGN.md section 5.4); mult: v's count in graph[c_k]
+int value_w_launch(long long n_node, int ld, const float *emb, const float *bias, const long long *raw_indptr,
+                   long long n_roots, const int *roots, const double *dist, const int *root_ok, const int *mult, double *W,
+                   cudaStream_t st);
 
 }  // namespace gg

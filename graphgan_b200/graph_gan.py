@@ -145,6 +145,14 @@ class GraphGAN(object):
         g, d = self.generator, self.discriminator
         return self.sampler.game_value_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
 
+    def game_value_grad_d(self, roots):
+        """game_value(roots) and the exact gradient of sum_{ok c} V_c with respect to the discriminator's padded rows and
+        biases (DESIGN.md section 5.4): sampler.WalkSampler.game_value_grad_d.  Returns device (pos, neg, ok, grad_emb fp64
+        [N, ld], grad_bias fp64 [N]); pos, neg and ok are the bits of game_value."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        return self.sampler.game_value_grad_d(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
+
     def _trees_of(self, roots):
         """the trees of ``roots``: rows of the resident trees when they hold every one of them, else built"""
         t = self.trees
@@ -175,10 +183,18 @@ class GraphGAN(object):
     def value_line(self):
         """The line evaluation() appends: "value:<mean V> pos:<mean pos> neg:<mean neg> roots:<ok roots>", the means taken
         over the ok roots of value_roots() (nan when there are none).  With config.value_grad, " gnorm:<norm>" follows:
-        the 2-norm of the gradient of the mean V over (E_G[:, :n_emb], b_G), exact (game_value_grad)."""
-        if getattr(config, "value_grad", False):
+        the 2-norm of the gradient of the mean V over (E_G[:, :n_emb], b_G), exact (game_value_grad).  With
+        config.value_grad_d, " dnorm:<norm>" comes last: the same for the discriminator, over (E_D[:, :n_emb], b_D)
+        (game_value_grad_d)."""
+        vg, vd = getattr(config, "value_grad", False), getattr(config, "value_grad_d", False)
+        if vg:
             pos, neg, ok, g_emb, g_bias = self.game_value_grad(self.value_roots())
-        else:
+        if vd:
+            out = self.game_value_grad_d(self.value_roots())
+            d_emb, d_bias = out[3:]
+            if not vg:
+                pos, neg, ok = out[:3]
+        if not (vg or vd):
             pos, neg, ok = self.game_value(self.value_roots())
         pos, neg, ok = (x.cpu().numpy() for x in (pos, neg, ok))
         sel = ok == 1
@@ -188,6 +204,9 @@ class GraphGAN(object):
         if getattr(config, "value_grad", False):
             sq = float((g_emb[:, :self.generator.n_emb] ** 2).sum().item() + (g_bias ** 2).sum().item())
             line += " gnorm:%r" % (float(np.sqrt(sq) / n) if n else np.nan)
+        if vd:
+            sq = float((d_emb[:, :self.discriminator.n_emb] ** 2).sum().item() + (d_bias ** 2).sum().item())
+            line += " dnorm:%r" % (float(np.sqrt(sq) / n) if n else np.nan)
         return line + "\n"
 
     def _next_tag(self):

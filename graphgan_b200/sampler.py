@@ -332,10 +332,12 @@ class WalkSampler:
             d.edge_score, d.hub_threshold = ptr(g.edge_score), self.hub_threshold
         return d
 
-    def _distribution_chunks(self, emb, bias, trees, reuse, max_scratch_bytes, counters, dist=None, root_ok=None):
+    def _distribution_chunks(self, emb, bias, trees, reuse, max_scratch_bytes, counters, dist=None, root_ok=None,
+                             extra_bytes=None):
         """gg_generator_dist over the roots of ``trees`` in chunks whose scratch fits the budget; yields (lo, hi, dist rows,
         root_ok rows) per chunk.  The rows go to dist[lo:hi] / root_ok[lo:hi] when those are given, else to one chunk-sized
-        buffer that the next chunk overwrites."""
+        buffer that the next chunk overwrites.  ``extra_bytes(k)``: the caller's own scratch for a chunk of k roots, counted
+        against the same budget (None: nothing)."""
         torch, g = self.torch, self.g
         R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
         if R == 0:
@@ -348,7 +350,8 @@ class WalkSampler:
             nb = C.c_int64(0)
             _cabi.check(self.lib.gg_generator_dist_scratch_bytes(N, nnz, k, C.byref(nb)), "gg_generator_dist_scratch_bytes")
             return nb.value
-        chunk = max(1, min(R, budget // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        per_root = scratch_bytes(1) + (extra_bytes(1) if extra_bytes is not None else 0)
+        chunk = max(1, min(R, budget // max(per_root, 1), ((1 << 31) - 1) // max(N, 1)))
         scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
         if dist is None:
             dist = torch.empty((chunk, N), dtype=torch.float64, device=self.device)
@@ -438,6 +441,59 @@ class WalkSampler:
             _cabi.check(self.lib.gg_game_value_grad(C.byref(d), ptr(d_emb), ptr(d_bias), ptr(g.raw_indptr), ptr(g.raw_adj),
                                                     ptr(sp[lo:hi]), ptr(sn[lo:hi]), ptr(so[lo:hi]), ptr(grad_emb),
                                                     ptr(grad_bias), ptr(scratch), scratch.numel(), st), "gg_game_value_grad")
+        pos[order], neg[order], ok[order] = sp, sn, so
+        return pos, neg, ok, grad_emb, grad_bias
+
+    # ------------------------------------------------------------------ discriminator gradient of V(G, D)
+    def game_value_grad_d(self, g_emb, g_bias, d_emb, d_bias, trees, *, max_scratch_bytes=None, reuse=None):
+        """``game_value`` and the exact gradient of sum_{ok c} V_c with respect to the discriminator's parameters (csrc/
+        value_dgrad.cu, DESIGN.md section 5.4): the expectation of the reference's D-step gradient (discriminator.py:26-30)
+        with the raw neighbours as positives and G-mode negatives, negated, without the L2 term.  D ascends V, so this is
+        the direction in which D improves.
+        Returns device (pos fp64 [R], neg fp64 [R], ok int32 [R]) in the order of ``trees`` -- the bits of ``game_value``
+        -- and (grad_emb fp64 [N, ld], grad_bias fp64 [N]) for the padded rows ``d_emb`` (pad columns exactly 0) and
+        ``d_bias``.  The roots are taken in ascending id order (stable for duplicates), in the chunks of ``distribution``
+        with this gradient's scratch counted against the same budget (``max_scratch_bytes``, default 2 GiB or env
+        GG_GDIST_SCRATCH), each coordinate one fp64 chain over the roots: the bits do not depend on the chunking, the order
+        of the roots or the call."""
+        torch, g = self.torch, self.g
+        assert d_emb.dtype == torch.float32 and d_emb.is_contiguous() and d_bias.dtype == torch.float32
+        assert int(d_emb.shape[0]) == g.n_node and int(d_bias.shape[0]) == g.n_node
+        R, N, ld = int(trees.roots.shape[0]), g.n_node, int(d_emb.shape[1])
+        pos = torch.zeros(R, dtype=torch.float64, device=self.device)
+        neg = torch.zeros(R, dtype=torch.float64, device=self.device)
+        ok = torch.zeros(R, dtype=torch.int32, device=self.device)
+        grad_emb = torch.zeros(tuple(d_emb.shape), dtype=torch.float64, device=self.device)
+        grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
+        if R == 0:
+            return pos, neg, ok, grad_emb, grad_bias
+        order = torch.argsort(trees.roots.long(), stable=True)
+        st_trees = trees.select(order)
+
+        def value_bytes(k):
+            nb = C.c_int64(0)
+            _cabi.check(self.lib.gg_game_value_scratch_bytes(N, k, C.byref(nb)), "gg_game_value_scratch_bytes")
+            return nb.value
+
+        def grad_bytes(k):
+            nb = C.c_int64(0)
+            _cabi.check(self.lib.gg_game_value_grad_d_scratch_bytes(N, ld, k, C.byref(nb)),
+                        "gg_game_value_grad_d_scratch_bytes")
+            return nb.value
+        sp, sn, so = (torch.zeros_like(x) for x in (pos, neg, ok))
+        st, vs, ds = self._stream(), None, None
+        for lo, hi, dist, root_ok in self._distribution_chunks(g_emb, g_bias, st_trees, reuse, max_scratch_bytes, None,
+                                                               extra_bytes=lambda k: value_bytes(k) + grad_bytes(k)):
+            if vs is None:                                              # the first chunk is the largest
+                vs = torch.empty(max(value_bytes(hi - lo), 16), dtype=torch.uint8, device=self.device)
+                ds = torch.empty(max(grad_bytes(hi - lo), 16), dtype=torch.uint8, device=self.device)
+            roots = st_trees.roots[lo:hi]
+            _cabi.check(self.lib.gg_game_value(N, ld, ptr(d_emb), ptr(d_bias), ptr(g.raw_indptr), ptr(g.raw_adj), hi - lo,
+                                               ptr(roots), ptr(dist), ptr(root_ok), ptr(sp[lo:hi]), ptr(sn[lo:hi]),
+                                               ptr(so[lo:hi]), ptr(vs), vs.numel(), st), "gg_game_value")
+            _cabi.check(self.lib.gg_game_value_grad_d(N, ld, ptr(d_emb), ptr(d_bias), ptr(g.raw_indptr), ptr(g.raw_adj),
+                                                      hi - lo, ptr(roots), ptr(dist), ptr(root_ok), ptr(grad_emb),
+                                                      ptr(grad_bias), ptr(ds), ds.numel(), st), "gg_game_value_grad_d")
         pos[order], neg[order], ok[order] = sp, sn, so
         return pos, neg, ok, grad_emb, grad_bias
 

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 9   /* 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
+#define GG_ABI_VERSION 10  /* 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -212,6 +212,24 @@ int gg_game_value_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_root
 int gg_game_value_grad(const gg_walk_desc *g, const float *d_emb, const float *d_bias, const int64_t *raw_indptr,
                        const int32_t *raw_adj, double *pos, double *neg, int32_t *ok, double *grad_emb, double *grad_bias,
                        void *scratch, int64_t scratch_bytes, void *stream);
+
+/* The exact discriminator gradient of the game value (csrc/value_dgrad.cu, DESIGN.md section 5.4): for the roots, dist and
+ * root_ok of gg_game_value (the other arguments as there), ADDS the gradient of sum_{ok c} V_c with respect to the
+ * discriminator's padded rows (emb, ld columns) and biases into grad_emb (device fp64 [n_node, ld]) and grad_bias (device
+ * fp64 [n_node]):
+ *   W[k, v] = dV_c / ds(c, v) = n_kv sigma(-s) / |graph[c]| - dist[k, v] sigma(s)   (c = roots[k], s the canonical fp32
+ *   score of gg_game_value, sigma in fp64; n_kv the count of v in the raw list graph[c], duplicates and self-loops too),
+ *   grad_bias[v] += W[k, v],  grad_emb[v] += W[k, v] emb[c],  grad_emb[c] += sum_v W[k, v] emb[v]
+ * for ok[k] = 1 only (the ok of gg_game_value); lambda_dis is not included.  Pad columns receive exactly 0.  Each node's
+ * row takes the roots in the order given as one fp64 chain per coordinate, continued from the value already in grad_emb /
+ * grad_bias: pass the roots in ascending id order (and chunks in order) for bits that do not depend on the order or the
+ * chunking.  scratch: device, at least gg_game_value_grad_d_scratch_bytes(n_node, ld, n_roots) bytes (host-only size
+ * computation; 12 bytes per (root, node) plus 8 ld bytes per root and 2048 nodes).  Five launches and one memset. */
+int gg_game_value_grad_d_scratch_bytes(int64_t n_node, int32_t ld, int64_t n_roots, int64_t *bytes);
+int gg_game_value_grad_d(int64_t n_node, int32_t ld, const float *emb, const float *bias, const int64_t *raw_indptr,
+                         const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist,
+                         const int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes,
+                         void *stream);
 
 /* prepare_data_for_d's output rows (graph_gan.py:192-201): for every accepted root, in batch
  * order: [i]*k + [i]*k | pos + neg | 1*k + 0*k.  row_ptr: device [R+1] scratch/out (exclusive
