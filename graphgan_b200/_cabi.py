@@ -9,7 +9,7 @@ import os
 from . import _build
 
 _LIB = None
-ABI_VERSION = 10    # == GG_ABI_VERSION of include/graphgan_b200.h
+ABI_VERSION = 11   # == GG_ABI_VERSION of include/graphgan_b200.h
 
 
 class GGError(RuntimeError):
@@ -92,6 +92,7 @@ SIGNATURES = {
                                       _I32, _P]),
     "gg_set_adam_path": (C.c_int, [C.c_char_p]),
     "gg_adam_apply": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _F, _F, _F, _F, _P]),
+    "gg_adam_apply_dense": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_double, _F, _F, _F, _F, _F, _F, _P]),
     "gg_train_steps": (C.c_int, [_I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P,
                                 _F, _F, _F, _F, C.POINTER(C.c_float), C.POINTER(C.c_float), _P]),
     "gg_train_steps_ex": (C.c_int, [_I32, _I64, _P, _I64, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _P, _P,

@@ -11,6 +11,7 @@
 // chains of the update are what the warps wait on -- ncu: fixed-latency dependency stalls -- so occupancy beats
 // deeper unrolling: 4 in flight at 112 registers ran at 45 % of DRAM peak); the row -> gradient-slot map
 // written by gg_pair_grad tells whether the row has a gradient, and is reset here.
+#include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -269,6 +270,95 @@ adam_ws_kernel(long long n_node, int ld, float *__restrict__ emb, float *__restr
     }
 }
 
+// ---------------------------------------------------------------- dense-gradient step of the exact game (DESIGN.md 5.5)
+// The sweep of adam_rows with a gradient for every element: the fp64 accumulators that gg_game_value_grad{,_d} fill,
+// g = f32(scale * acc + lambda * x) in fp64 (mul, mul, add: no contraction), then the GG_ADAM1 sequence.  A pure stream
+// of 32 bytes per element (acc 8, E / m / v 24).  A warp owns segments of 32 float4 (the element order of adam_rows)
+// and keeps UNR of them in flight; the lane holding a row's first columns also steps the row's bias.
+template <int UNR>
+__device__ __forceinline__ void adam_dense_rows(long long n_node, int ld, float *emb, float *m_emb, float *v_emb,
+                                                float *bias, float *m_bias, float *v_bias, const double *acc_emb,
+                                                const double *acc_bias, double scale, float lam_e, float lam_b,
+                                                float lr_t, float b1, float b2, float eps) {
+    const int lane = threadIdx.x & 31;
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+    const float omb1 = 1.0f - b1, omb2 = 1.0f - b2;
+    const int q = ld >> 2, qs = __ffs(q) - 1;     // float4 per row (a power of two) and its log2
+    const long long n4 = n_node * q;              // float4 in the whole matrix
+    const long long nseg = (n4 + 31) >> 5;
+    const double le = (double)lam_e, lb = (double)lam_b;
+#define GG_DENSE_G(a, xx) __double2float_rn(__dadd_rn(__dmul_rn(scale, (a)), __dmul_rn(le, (double)(xx))))
+#define GG_ADAM1(f)                                                                                   \
+    m[k].f = __fadd_rn(__fmul_rn(m[k].f, b1), __fmul_rn(omb1, g.f));                                  \
+    v[k].f = __fadd_rn(__fmul_rn(v[k].f, b2), __fmul_rn(__fmul_rn(g.f, g.f), omb2));                  \
+    x[k].f = __fsub_rn(x[k].f, __fdiv_rn(__fmul_rn(lr_t, m[k].f), __fadd_rn(__fsqrt_rn(v[k].f), eps)));
+    for (long long s0 = warp * UNR; s0 < nseg; s0 += nwarps * UNR) {
+        long long e4[UNR];                         // my float4 of segment s0 + k, or -1
+        float4 m[UNR], v[UNR], x[UNR];
+        double2 a0[UNR], a1[UNR];
+#pragma unroll
+        for (int k = 0; k < UNR; ++k) {
+            const long long e = ((s0 + k) << 5) + lane;
+            e4[k] = (s0 + k < nseg && e < n4) ? e : -1;
+            if (e4[k] >= 0) {
+                const size_t at = (size_t)e << 2;
+                m[k] = *reinterpret_cast<const float4 *>(m_emb + at);
+                v[k] = *reinterpret_cast<const float4 *>(v_emb + at);
+                x[k] = *reinterpret_cast<const float4 *>(emb + at);
+                a0[k] = __ldg(reinterpret_cast<const double2 *>(acc_emb + at));
+                a1[k] = __ldg(reinterpret_cast<const double2 *>(acc_emb + at + 2));
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < UNR; ++k) {
+            if (e4[k] < 0) continue;
+            const size_t at = (size_t)e4[k] << 2;
+            float4 g;
+            g.x = GG_DENSE_G(a0[k].x, x[k].x); g.y = GG_DENSE_G(a0[k].y, x[k].y);
+            g.z = GG_DENSE_G(a1[k].x, x[k].z); g.w = GG_DENSE_G(a1[k].y, x[k].w);
+            GG_ADAM1(x) GG_ADAM1(y) GG_ADAM1(z) GG_ADAM1(w)
+            *reinterpret_cast<float4 *>(m_emb + at) = m[k];
+            *reinterpret_cast<float4 *>(v_emb + at) = v[k];
+            *reinterpret_cast<float4 *>(emb + at) = x[k];
+            if ((e4[k] & (q - 1)) == 0) {          // this lane holds the row's first columns: the bias
+                const long long row = e4[k] >> qs;
+                const float xb = bias[row];
+                const float gb = __double2float_rn(__dadd_rn(__dmul_rn(scale, __ldg(acc_bias + row)), __dmul_rn(lb, (double)xb)));
+                const float mm = __fadd_rn(__fmul_rn(m_bias[row], b1), __fmul_rn(omb1, gb));
+                const float vv = __fadd_rn(__fmul_rn(v_bias[row], b2), __fmul_rn(__fmul_rn(gb, gb), omb2));
+                m_bias[row] = mm; v_bias[row] = vv;
+                bias[row] = __fsub_rn(xb, __fdiv_rn(__fmul_rn(lr_t, mm), __fadd_rn(__fsqrt_rn(vv), eps)));
+            }
+        }
+    }
+#undef GG_ADAM1
+#undef GG_DENSE_G
+}
+
+__global__ void __launch_bounds__(256, 4) adam_dense_kernel(long long n_node, int ld, float *__restrict__ emb,
+                                                         float *__restrict__ m_emb, float *__restrict__ v_emb,
+                                                         float *__restrict__ bias, float *__restrict__ m_bias,
+                                                         float *__restrict__ v_bias, const double *__restrict__ acc_emb,
+                                                         const double *__restrict__ acc_bias, double scale, float lam_e,
+                                                         float lam_b, float lr_t, float b1, float b2, float eps) {
+    adam_dense_rows<2>(n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, acc_emb, acc_bias, scale, lam_e, lam_b, lr_t,
+                       b1, b2, eps);
+}
+
+// ld = 512 as adam_wide_kernel: a warp keeps four segments -- one whole row -- in flight, at 2 CTAs per SM.
+__global__ void __launch_bounds__(256, 2) adam_dense_wide_kernel(long long n_node, int ld, float *__restrict__ emb,
+                                                              float *__restrict__ m_emb, float *__restrict__ v_emb,
+                                                              float *__restrict__ bias, float *__restrict__ m_bias,
+                                                              float *__restrict__ v_bias,
+                                                              const double *__restrict__ acc_emb,
+                                                              const double *__restrict__ acc_bias, double scale,
+                                                              float lam_e, float lam_b, float lr_t, float b1, float b2,
+                                                              float eps) {
+    adam_dense_rows<ADAM_WIDE_UNR>(n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, acc_emb, acc_bias, scale, lam_e,
+                                   lam_b, lr_t, b1, b2, eps);
+}
+
 // which sweep gg_adam_apply launches: 0 = per-thread loads (default: fastest measured), 1..3 = CTA-barrier TMA pipeline
 // (512x2, 256x2, 512x3 threads x CTAs per SM), 4 / 5 = warp-specialised TMA pipeline with 16 / 8 consumer warps
 int g_adam_path = -1;
@@ -350,4 +440,28 @@ extern "C" int gg_adam_apply(int64_t n_node, int32_t ld, float *emb, float *m_em
                                                                         v_bias, grad_rows, grad_bias, row_slot, lr_t,
                                                                         beta1, beta2, eps);
     return gg::check_cuda(cudaGetLastError(), "adam kernel launch");
+}
+
+extern "C" int gg_adam_apply_dense(int64_t n_node, int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias,
+                                   float *m_bias, float *v_bias, const double *acc_emb, const double *acc_bias,
+                                   double scale, float lambda_emb, float lambda_bias, float lr_t, float beta1,
+                                   float beta2, float eps, void *stream) {
+    GG_REQUIRE(emb && m_emb && v_emb && bias && m_bias && v_bias && acc_emb && acc_bias, "null pointer");
+    GG_REQUIRE(n_node > 0, "n_node must be positive");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
+    GG_REQUIRE(isfinite(scale), "scale must be finite");
+    const long long nseg = (n_node * (ld / 4) + 31) / 32;                      // 512-byte segments
+    const int unr = ld == gg::LD_MAX ? gg::ADAM_WIDE_UNR : 2;
+    long long blocks = (nseg + unr * 8 - 1) / (unr * 8);                         // 8 warps x unr segments in flight
+    const long long cap = (long long)gg::sm_count() * 16;
+    if (blocks > cap) blocks = cap;
+    if (ld == gg::LD_MAX)
+        gg::adam_dense_wide_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+            n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, acc_emb, acc_bias, scale, lambda_emb, lambda_bias, lr_t,
+            beta1, beta2, eps);
+    else
+        gg::adam_dense_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
+            n_node, ld, emb, m_emb, v_emb, bias, m_bias, v_bias, acc_emb, acc_bias, scale, lambda_emb, lambda_bias, lr_t,
+            beta1, beta2, eps);
+    return gg::check_cuda(cudaGetLastError(), "adam (dense gradient) kernel launch");
 }

@@ -30,6 +30,14 @@ from . import _cabi
 import ctypes as C
 
 
+def check_exact_mode(cfg, world):
+    """Refuse exact-game training (cfg.exact_roots > 0, DESIGN.md section 5.5) in a run of more than one process: its
+    steps are single-process."""
+    if getattr(cfg, "exact_roots", 0) > 0 and world > 1:
+        raise ValueError("config.exact_roots = %d trains on one process only, not %d (set exact_roots = 0 under torchrun)"
+                         % (cfg.exact_roots, world))
+
+
 def _device():
     dev = config.device
     if "LOCAL_RANK" in os.environ and str(dev).startswith("cuda"):
@@ -79,6 +87,7 @@ class GraphGAN(object):
         self.shuffle_rng = np.random.RandomState(config.seed)
         self.pass_counter = 0
         self.last_counters = {}
+        self.exact_trace = []                   # (phase, step, mean V, n_ok) of every exact step (config.exact_roots > 0)
         # one process per GPU: roots are sharded, rows all-gathered, updates data parallel (parallel.py)
         import torch.distributed as dist
         self.dist = dist if (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1) else None
@@ -209,6 +218,77 @@ class GraphGAN(object):
             line += " dnorm:%r" % (float(np.sqrt(sq) / n) if n else np.nan)
         return line + "\n"
 
+    # ------------------------------------------------------------------ training on the exact game (DESIGN.md section 5.5)
+    def exact_roots(self):
+        """The roots of exact training: config.exact_roots non-isolated roots seeded by config.seed (all of them when
+        exact_roots reaches their number), fixed for the run."""
+        key = (int(config.exact_roots), int(config.seed))
+        if getattr(self, "_exact_key", None) != key:
+            from . import synth
+            self._exact_roots = synth.pick_roots(self.host_graph.degrees(), key[0], seed=key[1])
+            self._exact_key = key
+        return self._exact_roots
+
+    def _exact_trees(self, roots):
+        """the trees of ``roots``, taken from the resident trees or built, once: they do not change during a run"""
+        key = roots.tobytes()
+        if getattr(self, "_exact_tree_key", None) != key:
+            self._exact_tree_cache, self._exact_tree_key = self._trees_of(roots), key
+        return self._exact_tree_cache
+
+    def exact_d_step(self, roots, *, law=None, max_scratch_bytes=None):
+        """One Adam step of the discriminator on the exact gradient of the mean game value over the ok roots of ``roots``:
+        game_value_grad_d, then apply_dense_grad with scale -1/n_ok (D ascends V; the L2 term is the model's own).
+        ``law``: the generator's law for these roots (sampler.WalkSampler.distribution of their trees), reused instead of
+        recomputed.  A step without ok roots changes nothing.  Returns the pre-step device (pos, neg, ok)."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        pos, neg, ok, gE, gb = self.sampler.game_value_grad_d(g.emb, g.bias_t, d.emb, d.bias_t, self._exact_trees(roots),
+                                                              max_scratch_bytes=max_scratch_bytes, law=law)
+        n_ok = int(ok.sum().item())
+        if n_ok:
+            d.apply_dense_grad(gE, gb, -1.0 / n_ok)
+        return pos, neg, ok
+
+    def exact_g_step(self, roots, *, max_scratch_bytes=None):
+        """One Adam step of the generator on the exact gradient of the mean game value over the ok roots of ``roots``:
+        game_value_grad, then apply_dense_grad with scale +1/n_ok (G descends V).  A step without ok roots changes nothing.
+        Returns the pre-step device (pos, neg, ok)."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        pos, neg, ok, gE, gb = self.sampler.game_value_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._exact_trees(roots),
+                                                            max_scratch_bytes=max_scratch_bytes)
+        n_ok = int(ok.sum().item())
+        if n_ok:
+            g.apply_dense_grad(gE, gb, 1.0 / n_ok)
+        return pos, neg, ok
+
+    def exact_d_phase(self, roots, steps, *, max_scratch_bytes=None):
+        """``steps`` exact D steps.  G is fixed meanwhile, so its law over the roots is computed once when it fits the
+        scratch budget of the exact-game entry points (8 bytes per root and node; ``max_scratch_bytes``, default env
+        GG_GDIST_SCRATCH or 2 GiB), else recomputed by every step -- the same bits either way.  Returns the steps' pre-step
+        (pos, neg, ok)."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        law = None
+        if steps > 0 and roots.shape[0] * self.n_node * 8 <= self.sampler.scratch_budget(max_scratch_bytes):
+            law = self.sampler.distribution(self.generator.emb, self.generator.bias_t, self._exact_trees(roots),
+                                            max_scratch_bytes=max_scratch_bytes)
+        return [self.exact_d_step(roots, law=law, max_scratch_bytes=max_scratch_bytes) for _ in range(steps)]
+
+    def _exact_phase(self, phase, outs):
+        """append the steps of one phase to exact_trace and print the phase's line"""
+        vals = []
+        for step, (pos, neg, ok) in enumerate(outs):
+            pos, neg, ok = (x.cpu().numpy() for x in (pos, neg, ok))
+            sel = ok == 1
+            n = int(sel.sum())
+            v = float((pos + neg)[sel].mean()) if n else float("nan")
+            self.exact_trace.append((phase, step, v, n))
+            vals.append(v)
+        if vals:
+            print("exact %s: %d steps, mean V %r -> %r before the first / last step, %d roots"
+                  % (phase, len(vals), vals[0], vals[-1], self.exact_trace[-1][3]))
+
     def _next_tag(self):
         self.pass_counter += 1
         return self.pass_counter
@@ -303,6 +383,8 @@ class GraphGAN(object):
 
     # ------------------------------------------------------------------ graph_gan.py:122-180
     def train(self):
+        check_exact_mode(config, self.world)
+        exact = config.exact_roots > 0
         torch = self.torch
         ckpt = os.path.join(config.model_log, "model.checkpoint.pt")
         if config.load_model and os.path.isfile(ckpt):
@@ -315,6 +397,13 @@ class GraphGAN(object):
             print("epoch %d" % epoch)
             if epoch > 0 and epoch % config.save_steps == 0:
                 self.save(ckpt)
+            if exact:       # full-expectation steps on V(G, D): no walks, so no removal bits, passes or shuffles change
+                roots = self.exact_roots()
+                self._exact_phase("D", self.exact_d_phase(roots, config.n_epochs_dis))
+                self._exact_phase("G", [self.exact_g_step(roots) for _ in range(config.n_epochs_gen)])
+                self.write_embeddings_to_file()
+                self.evaluation(self)
+                continue
             # D-steps
             center_nodes = neighbor_nodes = labels = None
             for d_epoch in range(config.n_epochs_dis):

@@ -198,6 +198,27 @@ class PairModel:
         self.beta2_power = np.float32(self.beta2_power * self.beta2)
         self.step_count += 1
 
+    def apply_dense_grad(self, acc_emb, acc_bias, scale):
+        """One Adam step from a dense fp64 gradient (DESIGN.md section 5.5): g = f32(scale * acc + lam * x) per element,
+        with ``acc_emb`` fp64 [N, ld] and ``acc_bias`` fp64 [N] as game_value_grad / game_value_grad_d return them.  The
+        L2 term is the model's own: lam on every row, and on every bias for the discriminator only (generator.py:28-29 has
+        no bias L2).  Shares lr_t, the beta powers and step_count with apply_adam, so sampled and exact steps continue one
+        Adam state."""
+        torch = self.torch
+        for a, shape in ((acc_emb, (self.n_node, self.ld)), (acc_bias, (self.n_node,))):
+            if a.dtype != torch.float64 or tuple(a.shape) != shape or not a.is_contiguous() or a.device != self.emb.device:
+                raise ValueError("apply_dense_grad takes contiguous fp64 device gradients of shape %s" % (shape,))
+        lam_b = self.lam if self._step_mode == 0 else np.float32(0)
+        _cabi.check(self.lib.gg_adam_apply_dense(self.n_node, self.ld, ptr(self.emb), ptr(self.m_emb), ptr(self.v_emb),
+                                                 ptr(self.bias_t), ptr(self.m_bias), ptr(self.v_bias), ptr(acc_emb),
+                                                 ptr(acc_bias), C.c_double(float(scale)), C.c_float(float(self.lam)),
+                                                 C.c_float(float(lam_b)), C.c_float(float(self.lr_t())),
+                                                 C.c_float(float(self.beta1)), C.c_float(float(self.beta2)),
+                                                 C.c_float(float(self.eps)), self._stream()), "gg_adam_apply_dense")
+        self.beta1_power = np.float32(self.beta1_power * self.beta1)
+        self.beta2_power = np.float32(self.beta2_power * self.beta2)
+        self.step_count += 1
+
     # ------------------------------------------------------------------ fetches
     def reward_pairs(self, node_id, node_neighbor_id):
         """log(1 + exp(clip(score, -10, 10))) for M pairs -> device fp32 [M] (discriminator.py:33-34)."""

@@ -445,7 +445,36 @@ class WalkSampler:
         return pos, neg, ok, grad_emb, grad_bias
 
     # ------------------------------------------------------------------ discriminator gradient of V(G, D)
-    def game_value_grad_d(self, g_emb, g_bias, d_emb, d_bias, trees, *, max_scratch_bytes=None, reuse=None):
+    @staticmethod
+    def scratch_budget(max_scratch_bytes=None):
+        """The device bytes the exact-game entry points may hold at once: ``max_scratch_bytes``, else env GG_GDIST_SCRATCH,
+        else 2 GiB."""
+        return int(max_scratch_bytes if max_scratch_bytes is not None else os.environ.get("GG_GDIST_SCRATCH", 2 << 30))
+
+    def _given_law_chunks(self, law, order, max_scratch_bytes, extra_bytes):
+        """The chunks of ``_distribution_chunks`` for a law computed earlier: ``law = (dist [R, N], root_ok [R])`` from
+        ``distribution`` of the trees whose rows ``order`` selects.  Yields (lo, hi, dist rows, root_ok rows) of the roots
+        order[lo:hi]; the rows are gathered per chunk (8 N bytes per root, counted with ``extra_bytes`` against the budget)
+        unless ``order`` is the identity."""
+        torch = self.torch
+        dist, root_ok = law
+        R, N = int(order.shape[0]), self.g.n_node
+        if (dist.dtype != torch.float64 or tuple(dist.shape) != (R, N) or not dist.is_contiguous()
+                or root_ok.dtype != torch.int32 or tuple(root_ok.shape) != (R,)):
+            raise ValueError("law must be distribution's (dist fp64 [%d, %d], root_ok int32 [%d]) for the same trees"
+                             % (R, N, R))
+        ident = bool(torch.equal(order, torch.arange(R, device=order.device)))
+        per_root = extra_bytes(1) + (0 if ident else 8 * N)
+        chunk = max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(per_root, 1), ((1 << 31) - 1) // max(N, 1)))
+        for lo in range(0, R, chunk):
+            hi = min(R, lo + chunk)
+            if ident:
+                yield lo, hi, dist[lo:hi], root_ok[lo:hi]
+            else:
+                idx = order[lo:hi]
+                yield lo, hi, dist.index_select(0, idx), root_ok.index_select(0, idx)
+
+    def game_value_grad_d(self, g_emb, g_bias, d_emb, d_bias, trees, *, max_scratch_bytes=None, reuse=None, law=None):
         """``game_value`` and the exact gradient of sum_{ok c} V_c with respect to the discriminator's parameters (csrc/
         value_dgrad.cu, DESIGN.md section 5.4): the expectation of the reference's D-step gradient (discriminator.py:26-30)
         with the raw neighbours as positives and G-mode negatives, negated, without the L2 term.  D ascends V, so this is
@@ -455,7 +484,10 @@ class WalkSampler:
         ``d_bias``.  The roots are taken in ascending id order (stable for duplicates), in the chunks of ``distribution``
         with this gradient's scratch counted against the same budget (``max_scratch_bytes``, default 2 GiB or env
         GG_GDIST_SCRATCH), each coordinate one fp64 chain over the roots: the bits do not depend on the chunking, the order
-        of the roots or the call."""
+        of the roots or the call.
+        ``law``: ``distribution(g_emb, g_bias, trees)``'s (dist, root_ok), computed earlier for these same trees under the
+        same generator and removal bits; it is used instead of recomputing the law, with identical bits (DESIGN.md section
+        5.5: a D phase holds G fixed)."""
         torch, g = self.torch, self.g
         assert d_emb.dtype == torch.float32 and d_emb.is_contiguous() and d_bias.dtype == torch.float32
         assert int(d_emb.shape[0]) == g.n_node and int(d_bias.shape[0]) == g.n_node
@@ -482,8 +514,12 @@ class WalkSampler:
             return nb.value
         sp, sn, so = (torch.zeros_like(x) for x in (pos, neg, ok))
         st, vs, ds = self._stream(), None, None
-        for lo, hi, dist, root_ok in self._distribution_chunks(g_emb, g_bias, st_trees, reuse, max_scratch_bytes, None,
-                                                               extra_bytes=lambda k: value_bytes(k) + grad_bytes(k)):
+        extra = lambda k: value_bytes(k) + grad_bytes(k)
+        if law is None:
+            chunks = self._distribution_chunks(g_emb, g_bias, st_trees, reuse, max_scratch_bytes, None, extra_bytes=extra)
+        else:
+            chunks = self._given_law_chunks(law, order, max_scratch_bytes, extra)
+        for lo, hi, dist, root_ok in chunks:
             if vs is None:                                              # the first chunk is the largest
                 vs = torch.empty(max(value_bytes(hi - lo), 16), dtype=torch.uint8, device=self.device)
                 ds = torch.empty(max(grad_bytes(hi - lo), 16), dtype=torch.uint8, device=self.device)

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 10  /* 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
+#define GG_ABI_VERSION 11  /* 11: gg_adam_apply_dense; 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -401,6 +401,17 @@ int gg_adam_apply(int64_t n_node, int32_t ld, float *emb, float *m_emb, float *v
                   float *m_bias, float *v_bias, const int32_t *n_unique, const int32_t *uniq_ids,
                   const float *grad_rows, const float *grad_bias, int32_t *row_slot, float lr_t,
                   float beta1, float beta2, float eps, void *stream);
+
+/* The same TF1.8 Adam step from a dense fp64 gradient (the exact game's steps, DESIGN.md section 5.5): acc_emb
+ * [n_node, ld] and acc_bias [n_node] as gg_game_value_grad / gg_game_value_grad_d fill them.  Per element
+ *     g = (float)(scale * acc + (double)lambda * (double)x)      fp64 mul, mul, add (no contraction), rounded once
+ * with lambda = lambda_emb for the rows and lambda_bias for the biases, then the m / v / variable sequence of
+ * gg_adam_apply for every row and every bias.  Pad columns (acc = x = 0) stay exactly 0.  Refuses NULL pointers,
+ * n_node <= 0, an unsupported ld and a non-finite scale.  One launch. */
+int gg_adam_apply_dense(int64_t n_node, int32_t ld, float *emb, float *m_emb, float *v_emb, float *bias,
+                        float *m_bias, float *v_bias, const double *acc_emb, const double *acc_bias,
+                        double scale, float lambda_emb, float lambda_bias, float lr_t,
+                        float beta1, float beta2, float eps, void *stream);
 
 /* The inner training loop of graph_gan.py:149-157 / 168-176: for each start in start_list (host array, already
  * shuffled by the caller): one optimizer step on rows [start, min(start + batch_size, n_rows)) of the device
