@@ -60,6 +60,8 @@ value_roots = 0                     # > 0: evaluation also writes "value:<V> pos
 value_grad = False                 # with value_roots > 0: the value line also ends in " gnorm:<|grad_G mean V|_2>", exact
                                     # (DESIGN.md section 5.2) averaged over this many seeded roots (rank 0's shard under torchrun)
 value_grad_d = False               # with value_roots > 0: the value line ends in " dnorm:<|grad_D mean V|_2>", exact (section 5.4)
+value_gcos = False                 # with value_roots > 0: the value line ends in " gcos:<cos>", the cosine between the exact
+                                    # expectation of the reference's G step and grad_G V (DESIGN.md section 5.6)
 exact_roots = 0                     # > 0: train() plays the exact game on this many seeded roots (DESIGN.md section 5.5):
                                     # each D / G step is an Adam step on the exact gradient of the mean V; no walks are
                                     # sampled.  Single process only.  0: the reference's sampled training

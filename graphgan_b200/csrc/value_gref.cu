@@ -1,0 +1,447 @@
+// value_gref.cu -- the exact expectation of the reference's generator step (DESIGN.md section 5.6).
+//
+// The reference's G pass (graph_gan.py:204-223, generator.py:22-31) takes every ordered pair within `window` of each
+// walk's body and weights the pair's gradient by D's reward.  A G walk's body is the tree path root = a_0, ..., a_L = v
+// (the path without the father it stops on), so it holds y exactly when the walk reaches y, with probability
+//   reach(y) = fl(reach(father(y)) * pi_in(y)),  reach(root) = 1      (the section 5.1 chain, bit for bit)
+// and for every reached y != root at depth delta(y) and d = 1 .. min(w, delta(y)), x = anc_d(y), the ordered pairs (x, y)
+// and (y, x) each occur reach(y) times per walk.  Per pair (n1, n2), with the production bits:
+//   r     = log(1 + exp(clip(s_D(n1, n2), +-10)))                         (gg_pair_reward)
+//   kappa = -r (1 - p), p = sigmoid(s_G(n1, n2)); 0 when p < 1e-5f         (pair_delta mode 1, a_k = r, batch_total = 1)
+// and the expected per-walk gradient adds rho kappa E_G[n2] to grad_E[n1], rho kappa E_G[n1] to grad_E[n2] and rho kappa to
+// grad_b[n2] (rho = reach of the pair's deeper node).  kappa_up = kappa(x, y), kappa_dn = kappa(y, x) share one G dot and
+// one D dot (the canonical fma chain is symmetric in its operands); each direction adds its own bias.
+//
+// Per chunk of roots: the recording section 5.1 kernel (gdist.cu); reach_kernel, top-down over the recorded levels;
+// score_kernel, an 8-lane group per (item, d), writes kappa_up / kappa_dn into fp32 planes [w][R, N] indexed by the deeper
+// node; npairs_kernel, a CTA per root; gather_kernel adds each root's contribution to each row.
+//
+// Order (the bits depend on the inputs only): a node's row takes the roots in the order given (WalkSampler sorts them by
+// id), one fp64 chain per coordinate continued from the caller's accumulator.  A root's contribution to node a is
+//   up + (((chain_0 + chain_1) + ...) + chain_7)
+// where `up` runs over d = 1 .. min(w, delta(a)) (a as the deeper node) and chain_q, from +0, over the children of a at
+// entries a0 + 256 (q + 8 m) + [0, 256) in entry order, each child followed by its reached descendants within w levels of
+// a in depth-first pre-order, children in entry order (a as the ancestor).  A list of at most 256 entries has chain_0 only.
+// Every term is one fma per coordinate with c = fl(rho * fl(kappa_up + kappa_dn)) (fp64), and one add of rho kappa for the
+// bias.
+#include <cooperative_groups.h>
+#include <math.h>
+
+#include "update_dev.cuh"
+#include "value_grad.cuh"
+#include "walk_common.cuh"
+
+namespace gg {
+namespace {
+
+namespace cg = cooperative_groups;
+
+constexpr int GR_THREADS = 256;
+constexpr int GR_CHAINS = GR_THREADS / 32;     // 8 chains, one per warp of a hub node's CTA
+constexpr long long GR_BLOCK = 256;            // entries per chain block; lists up to this length are one warp's item
+constexpr int GR_WMAX = 8;                     // the largest window
+
+struct GrArgs {
+    long long n_node, n_roots, tree_words, rn;
+    int ld, window;
+    const long long *indptr;
+    const int *adj, *roots, *ok;
+    const uint32_t *tree_bits;
+    const float *emb, *bias, *d_emb, *d_bias;
+    const double *pi_in;
+    double *reach;
+    const int *father;
+    const int4 *items;
+    const unsigned *lev_off, *n_lev;
+    float *kup, *kdn;                          // [window][n_roots, n_node]: kappa(anc_d(y), y), kappa(y, anc_d(y))
+    int *big;
+    unsigned *big_cnt;
+    double *n_pairs, *grad_emb, *grad_bias;
+};
+
+__device__ __forceinline__ bool tree_bit(const uint32_t *tb, long long e) { return (__ldg(tb + (e >> 5)) >> (e & 31)) & 1u; }
+
+__device__ __forceinline__ double warp_dsum(double x) {
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) x = __dadd_rn(x, __shfl_xor_sync(FULL, x, off));
+    return x;
+}
+
+// top-down over the recorded levels, a thread per item, one grid barrier per level
+__global__ void __launch_bounds__(GR_THREADS) reach_kernel(const GrArgs g) {
+    cg::grid_group grid = cg::this_grid();
+    const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+    const int n_lev = (int)*g.n_lev;
+    for (int lev = 0; lev < n_lev; ++lev) {
+        const long long i0 = g.lev_off[lev], i1 = g.lev_off[lev + 1];
+        for (long long i = i0 + tid; i < i1; i += nt) {
+            const int4 it = g.items[i];
+            if (__ldg(g.ok + it.x) != 1) continue;
+            const size_t o = (size_t)it.x * (size_t)g.n_node;
+            g.reach[o + it.y] = it.z < 0 ? 1.0 : __dmul_rn(g.reach[o + it.z], g.pi_in[o + it.y]);
+        }
+        grid.sync();
+    }
+}
+
+// the production reward and G coefficient of one pair from its dots (pairs.cu reward_kernel, update_dev.cuh pair_delta)
+__device__ __forceinline__ float pair_kappa(float dot_g, float b_g, float dot_d, float b_d) {
+    float sd = __fadd_rn(dot_d, b_d);
+    sd = fminf(fmaxf(sd, -10.0f), 10.0f);
+    const float r = logf(1.0f + expf(sd));
+    const float s = __fadd_rn(dot_g, b_g);
+    const float p = (float)(1.0 / (1.0 + exp(-(double)s)));
+    return (p >= 1e-5f) ? __fmul_rn(-r, __fsub_rn(1.0f, p)) : 0.0f;
+}
+
+// an 8-lane group per (item of depth >= 1, d): the canonical group dots of (anc_d(y), y) under G and D
+__global__ void __launch_bounds__(GR_THREADS) score_kernel(const GrArgs g) {
+    const int lane = threadIdx.x & 31, grp = lane >> 3, gl = lane & 7;
+    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = ((long long)gridDim.x * blockDim.x) >> 5;
+    const long long i0 = g.lev_off[1 < *g.n_lev ? 1 : *g.n_lev], i1 = g.lev_off[*g.n_lev];
+    const int per_item = (g.window + 3) / 4;                  // passes of 4 groups per item
+    for (long long w0 = gw; w0 < (i1 - i0) * per_item; w0 += nw) {
+        const int4 it = g.items[i0 + w0 / per_item];
+        const int d = (int)(w0 % per_item) * 4 + grp + 1;
+        const size_t o = (size_t)it.x * (size_t)g.n_node;
+        const int y = it.y;
+        int x = -1;
+        if (__ldg(g.ok + it.x) == 1 && d <= g.window) {
+            x = it.z;
+            for (int k = 1; k < d && x >= 0; ++k) x = g.father[o + x];
+        }
+        const int xx = x >= 0 ? x : y;                         // x < 0: y is shallower than d (the dots are warp-wide)
+        const float dg = group_dot_t<false>(g.emb + (size_t)xx * g.ld, g.emb + (size_t)y * g.ld, g.ld, gl);
+        const float dd = group_dot_t<false>(g.d_emb + (size_t)xx * g.ld, g.d_emb + (size_t)y * g.ld, g.ld, gl);
+        if (x < 0 || gl != 0) continue;
+        const size_t at = (size_t)(d - 1) * (size_t)g.rn + o + y;
+        g.kup[at] = pair_kappa(dg, __ldg(g.bias + y), dd, __ldg(g.d_bias + y));
+        g.kdn[at] = pair_kappa(dg, __ldg(g.bias + x), dd, __ldg(g.d_bias + x));
+    }
+}
+
+// min(w, depth of v) in root slot o (0 for the root and for nodes not reached)
+__device__ __forceinline__ int window_depth(const GrArgs &g, size_t o, int v) {
+    int x = g.father[o + v], m = 0;
+    while (x >= 0 && m < g.window) {
+        ++m;
+        x = g.father[o + x];
+    }
+    return m;
+}
+
+// n_pairs[k] = sum_v reach(v) 2 min(w, depth(v)): thread t chains v = t, t + 256, ..., then the warps' butterflies in
+// warp order
+__global__ void __launch_bounds__(GR_THREADS) npairs_kernel(const GrArgs g) {
+    __shared__ double s_w[GR_CHAINS];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    for (long long k = blockIdx.x; k < g.n_roots; k += gridDim.x) {
+        double s = 0.0;
+        if (__ldg(g.ok + k) == 1) {
+            const size_t o = (size_t)k * (size_t)g.n_node;
+            for (long long v = threadIdx.x; v < g.n_node; v += GR_THREADS) {
+                const int m = window_depth(g, o, (int)v);
+                if (m) s = __dadd_rn(s, __dmul_rn(g.reach[o + v], (double)(2 * m)));
+            }
+        }
+        s = warp_dsum(s);
+        if (lane == 0) s_w[wid] = s;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double t = s_w[0];
+            for (int q = 1; q < GR_CHAINS; ++q) t = __dadd_rn(t, s_w[q]);
+            g.n_pairs[k] = t;
+        }
+        __syncthreads();
+    }
+}
+
+__global__ void big_nodes_kernel(const GrArgs g) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= g.n_node) return;
+    if (__ldg(g.indptr + i + 1) - __ldg(g.indptr + i) > GR_BLOCK) g.big[atomicAdd(g.big_cnt, 1u)] = (int)i;
+}
+
+// the pair coefficient c = rho (kappa_up + kappa_dn) of (anc_d(y), y) and the bias term of its node side
+__device__ __forceinline__ double pair_coef(const GrArgs &g, size_t o, int y, int d, double &rho) {
+    const size_t at = (size_t)(d - 1) * (size_t)g.rn + o + y;
+    rho = g.reach[o + y];
+    return __dmul_rn(rho, __dadd_rn((double)g.kup[at], (double)g.kdn[at]));
+}
+
+// chain_q of node a in root slot o (see the top of the file): s[i] for coordinate lane + 32 i, sb for the bias.  A
+// warp-uniform depth-first walk: frame t holds a node at distance t from a, the window of 32 of its entries being visited
+// (mask: the reached children not yet taken) and the next window.
+template <int CPL>
+__device__ __forceinline__ void down_chain(const GrArgs &g, size_t o, const uint32_t *tb, int a, long long a0, long long a1,
+                                           int q, int lane, double (&s)[CPL], double &sb) {
+    constexpr int LD = 32 * CPL;
+#pragma unroll
+    for (int i = 0; i < CPL; ++i) s[i] = 0.0;
+    sb = 0.0;
+    int nd[GR_WMAX];
+    long long nxt[GR_WMAX], end[GR_WMAX], base[GR_WMAX];
+    unsigned msk[GR_WMAX];
+    for (long long b0 = a0 + GR_BLOCK * q; b0 < a1; b0 += GR_BLOCK * GR_CHAINS) {
+        int top = 0;
+        nd[0] = a; nxt[0] = b0; end[0] = b0 + GR_BLOCK < a1 ? b0 + GR_BLOCK : a1; msk[0] = 0u; base[0] = b0;
+        while (true) {
+            if (msk[top] == 0u) {
+                if (nxt[top] >= end[top]) {
+                    if (top == 0) break;
+                    --top;
+                    continue;
+                }
+                const long long e = nxt[top] + lane;
+                bool take = false;
+                if (e < end[top] && tree_bit(tb, e)) take = g.father[o + __ldg(g.adj + e)] == nd[top];
+                msk[top] = __ballot_sync(FULL, take);
+                base[top] = nxt[top];
+                nxt[top] += 32;
+                continue;
+            }
+            const int bit = __ffs(msk[top]) - 1;
+            msk[top] &= msk[top] - 1u;
+            const int y = __ldg(g.adj + base[top] + bit);
+            const int dist = top + 1;
+            double rho;
+            const double c = pair_coef(g, o, y, dist, rho);
+            sb = __dadd_rn(sb, __dmul_rn(rho, (double)g.kdn[(size_t)(dist - 1) * (size_t)g.rn + o + y]));
+#pragma unroll
+            for (int i = 0; i < CPL; ++i) s[i] = __fma_rn(c, (double)__ldg(g.emb + (size_t)y * LD + lane + 32 * i), s[i]);
+            if (dist < g.window) {
+                ++top;
+                nd[top] = y; nxt[top] = __ldg(g.indptr + y); end[top] = __ldg(g.indptr + y + 1); msk[top] = 0u;
+                base[top] = nxt[top];
+            }
+        }
+    }
+}
+
+// Work items: first one CTA per big node, then groups of 8 nodes, a warp per node (big nodes skipped).  Each item runs
+// the roots in order and stores its rows once.
+template <int CPL>
+__global__ void __launch_bounds__(GR_THREADS) gather_kernel(const GrArgs g) {
+    constexpr int LD = 32 * CPL;
+    extern __shared__ __align__(16) unsigned char gr_smem[];
+    double *s_ch = reinterpret_cast<double *>(gr_smem);   // [GR_CHAINS, LD] chain sums, then [GR_CHAINS] bias chains
+    double *s_chb = s_ch + GR_CHAINS * LD;
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const long long n_big = *g.big_cnt, n_groups = (g.n_node + GR_CHAINS - 1) / GR_CHAINS;
+    for (long long item = blockIdx.x; item < n_big + n_groups; item += gridDim.x) {
+        if (item < n_big) {
+            // ---- a big node: warp q runs chain_q; thread t owns coordinates t, t + 256
+            const int a = g.big[item];
+            const long long a0 = __ldg(g.indptr + a), a1 = __ldg(g.indptr + a + 1);
+            double acc[2], accb = 0.0;
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int j = threadIdx.x + GR_THREADS * r;
+                acc[r] = j < LD ? g.grad_emb[(size_t)a * LD + j] : 0.0;
+            }
+            if (threadIdx.x == 0) accb = g.grad_bias[a];
+            for (long long k = 0; k < g.n_roots; ++k) {
+                if (__ldg(g.ok + k) != 1) continue;
+                const size_t o = (size_t)k * (size_t)g.n_node;
+                const bool is_root = __ldg(g.roots + k) == a;
+                if (!is_root && g.father[o + a] < 0) continue;                 // not reached from this root
+                double s[CPL], sb;
+                down_chain<CPL>(g, o, g.tree_bits + (size_t)k * (size_t)g.tree_words, a, a0, a1, wid, lane, s, sb);
+#pragma unroll
+                for (int i = 0; i < CPL; ++i) s_ch[wid * LD + lane + 32 * i] = s[i];
+                if (lane == 0) s_chb[wid] = sb;
+                __syncthreads();
+                double up[2] = {0.0, 0.0}, upb = 0.0;
+                int x = is_root ? -1 : g.father[o + a];
+                for (int d = 1; d <= g.window && x >= 0; ++d) {
+                    double rho;
+                    const double c = pair_coef(g, o, a, d, rho);
+                    upb = __dadd_rn(upb, __dmul_rn(rho, (double)g.kup[(size_t)(d - 1) * (size_t)g.rn + o + a]));
+#pragma unroll
+                    for (int r = 0; r < 2; ++r) {
+                        const int j = threadIdx.x + GR_THREADS * r;
+                        if (j < LD) up[r] = __fma_rn(c, (double)__ldg(g.emb + (size_t)x * LD + j), up[r]);
+                    }
+                    x = g.father[o + x];
+                }
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    const int j = threadIdx.x + GR_THREADS * r;
+                    if (j >= LD) continue;
+                    double ch = s_ch[j];
+                    for (int q = 1; q < GR_CHAINS; ++q) ch = __dadd_rn(ch, s_ch[q * LD + j]);
+                    acc[r] = __dadd_rn(acc[r], __dadd_rn(up[r], ch));
+                }
+                if (threadIdx.x == 0) {
+                    double chb = s_chb[0];
+                    for (int q = 1; q < GR_CHAINS; ++q) chb = __dadd_rn(chb, s_chb[q]);
+                    accb = __dadd_rn(accb, __dadd_rn(upb, chb));
+                }
+                __syncthreads();
+            }
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int j = threadIdx.x + GR_THREADS * r;
+                if (j < LD) g.grad_emb[(size_t)a * LD + j] = acc[r];
+            }
+            if (threadIdx.x == 0) g.grad_bias[a] = accb;
+            continue;
+        }
+        // ---- a group of 8 nodes, a warp per node: chain_0 only
+        const long long a = (item - n_big) * GR_CHAINS + wid;
+        if (a >= g.n_node) continue;
+        const long long a0 = __ldg(g.indptr + a), a1 = __ldg(g.indptr + a + 1);
+        if (a1 - a0 > GR_BLOCK) continue;
+        double acc[CPL];
+#pragma unroll
+        for (int i = 0; i < CPL; ++i) acc[i] = g.grad_emb[(size_t)a * LD + lane + 32 * i];
+        double accb = g.grad_bias[a];
+        for (long long k = 0; k < g.n_roots; ++k) {
+            if (__ldg(g.ok + k) != 1) continue;
+            const size_t o = (size_t)k * (size_t)g.n_node;
+            const bool is_root = __ldg(g.roots + k) == (int)a;
+            if (!is_root && g.father[o + a] < 0) continue;
+            double s[CPL], sb;
+            down_chain<CPL>(g, o, g.tree_bits + (size_t)k * (size_t)g.tree_words, (int)a, a0, a1, 0, lane, s, sb);
+            double up[CPL], upb = 0.0;
+#pragma unroll
+            for (int i = 0; i < CPL; ++i) up[i] = 0.0;
+            int x = is_root ? -1 : g.father[o + a];
+            for (int d = 1; d <= g.window && x >= 0; ++d) {
+                double rho;
+                const double c = pair_coef(g, o, (int)a, d, rho);
+                upb = __dadd_rn(upb, __dmul_rn(rho, (double)g.kup[(size_t)(d - 1) * (size_t)g.rn + o + a]));
+#pragma unroll
+                for (int i = 0; i < CPL; ++i) up[i] = __fma_rn(c, (double)__ldg(g.emb + (size_t)x * LD + lane + 32 * i), up[i]);
+                x = g.father[o + x];
+            }
+#pragma unroll
+            for (int i = 0; i < CPL; ++i) acc[i] = __dadd_rn(acc[i], __dadd_rn(up[i], s[i]));
+            accb = __dadd_rn(accb, __dadd_rn(upb, sb));
+        }
+#pragma unroll
+        for (int i = 0; i < CPL; ++i) g.grad_emb[(size_t)a * LD + lane + 32 * i] = acc[i];
+        if (lane == 0) g.grad_bias[a] = accb;
+    }
+}
+
+template <int CPL>
+int launch_gather(const GrArgs &g, cudaStream_t st) {
+    const size_t smem = (size_t)GR_CHAINS * (32 * CPL + 1) * sizeof(double);
+    GG_CHECK(cudaFuncSetAttribute(gather_kernel<CPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gather_kernel<CPL>, GR_THREADS, smem));
+    GG_REQUIRE(per_sm >= 1, "expected G step gather kernel does not fit on an SM");
+    const long long n_groups = (g.n_node + GR_CHAINS - 1) / GR_CHAINS;
+    long long grid = (long long)sm_count() * per_sm;
+    if (grid > n_groups + g.n_node) grid = n_groups + g.n_node;
+    gather_kernel<CPL><<<(unsigned)grid, GR_THREADS, smem, st>>>(g);
+    return check_cuda(cudaGetLastError(), "expected G step gather launch");
+}
+
+struct GrLayout {
+    void *rec;                                 // gdist_rec_layout's part
+    double *dist, *reach, *pi_in, *pi_stop;
+    float *kup, *kdn;
+    int *father, *root_ok, *big;
+    unsigned *big_cnt;
+};
+
+size_t gr_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, int window, GrLayout *v) {
+    size_t off = 0;
+    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t rn = (size_t)n_roots * (size_t)n_node;
+    const size_t o_rec = take(gdist_rec_layout(nullptr, n_node, nnz_words, n_roots, nullptr));
+    const size_t o_dist = take(rn * sizeof(double)), o_reach = take(rn * sizeof(double));
+    const size_t o_pin = take(rn * sizeof(double)), o_pst = take(rn * sizeof(double));
+    const size_t o_kup = take((size_t)window * rn * sizeof(float)), o_kdn = take((size_t)window * rn * sizeof(float));
+    const size_t o_fa = take(rn * sizeof(int)), o_ok = take((size_t)n_roots * sizeof(int));
+    const size_t o_big = take((size_t)n_node * sizeof(int)), o_bc = take(sizeof(unsigned));
+    if (buf && v) {
+        unsigned char *b = static_cast<unsigned char *>(buf);
+        v->rec = b + o_rec;
+        v->dist = reinterpret_cast<double *>(b + o_dist);
+        v->reach = reinterpret_cast<double *>(b + o_reach);
+        v->pi_in = reinterpret_cast<double *>(b + o_pin);
+        v->pi_stop = reinterpret_cast<double *>(b + o_pst);
+        v->kup = reinterpret_cast<float *>(b + o_kup);
+        v->kdn = reinterpret_cast<float *>(b + o_kdn);
+        v->father = reinterpret_cast<int *>(b + o_fa);
+        v->root_ok = reinterpret_cast<int *>(b + o_ok);
+        v->big = reinterpret_cast<int *>(b + o_big);
+        v->big_cnt = reinterpret_cast<unsigned *>(b + o_bc);
+    }
+    return off;
+}
+
+}  // namespace
+}  // namespace gg
+
+extern "C" int gg_expected_g_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int32_t window,
+                                                int64_t *bytes) {
+    GG_REQUIRE(bytes && n_node >= 0 && nnz >= 0 && n_roots >= 0, "bad arguments");
+    GG_REQUIRE(window >= 1 && window <= gg::GR_WMAX, "window must be 1 .. 8");
+    *bytes = (int64_t)gg::gr_layout(nullptr, n_node, (nnz + 31) / 32, n_roots, window, nullptr);
+    return 0;
+}
+
+extern "C" int gg_expected_g_grad(const gg_walk_desc *gp, const float *d_emb, const float *d_bias, int32_t window,
+                                  double *n_pairs, int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch,
+                                  int64_t scratch_bytes, void *stream) {
+    GG_REQUIRE(gp, "null descriptor");
+    const gg_walk_desc &d = *gp;
+    GG_REQUIRE(gg::ld_supported(d.ld), GG_LD_MESSAGE);
+    GG_REQUIRE(window >= 1 && window <= gg::GR_WMAX, "window must be 1 .. 8");
+    GG_REQUIRE(d.n_roots >= 0, "n_roots must be >= 0");
+    if (d.n_roots == 0) return 0;
+    GG_REQUIRE(d.n_node > 0 && d.emb && d.bias && d.indptr && d.adj && d.roots && d.tree_bits, "null graph/embedding pointer");
+    GG_REQUIRE(d.tree_words > 0, "tree_words missing (gg_tree_words)");
+    GG_REQUIRE(d_emb && d_bias, "null discriminator pointer");
+    GG_REQUIRE(n_pairs && root_ok && grad_emb && grad_bias && scratch, "null output or scratch pointer");
+    GG_REQUIRE(d.n_roots * d.n_node < (1ll << 31), "n_roots * n_node must be below 2^31 (process the roots in chunks)");
+    GG_REQUIRE(!d.edge_score || (d.hub_threshold > 0 && d.hub_threshold < gg::SMEM_CAP), "hub_threshold out of range");
+    gg::GrLayout v;
+    const size_t need = gg::gr_layout(scratch, d.n_node, d.tree_words - 1, d.n_roots, window, &v);
+    GG_REQUIRE(scratch_bytes >= (int64_t)need, "scratch too small (gg_expected_g_grad_scratch_bytes)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t rn = (size_t)d.n_roots * (size_t)d.n_node;
+    GG_CHECK(cudaMemsetAsync(v.dist, 0, rn * sizeof(double), st));
+    GG_CHECK(cudaMemsetAsync(root_ok, 0, (size_t)d.n_roots * sizeof(int32_t), st));
+    GG_CHECK(cudaMemsetAsync(v.father, 0xff, rn * sizeof(int), st));
+    GG_CHECK(cudaMemsetAsync(v.big_cnt, 0, sizeof(unsigned), st));
+    gg::GdRec rec;
+    rec.pi_in = v.pi_in; rec.pi_stop = v.pi_stop; rec.father = v.father;
+    gg::gdist_rec_layout(v.rec, d.n_node, d.tree_words - 1, d.n_roots, &rec);
+    int rc = gg::gdist_rec_launch(d, v.dist, root_ok, rec, v.rec, st);
+    if (rc) return rc;
+    gg::GrArgs g;
+    g.n_node = d.n_node; g.n_roots = d.n_roots; g.tree_words = d.tree_words; g.rn = (long long)rn;
+    g.ld = d.ld; g.window = window;
+    g.indptr = (const long long *)d.indptr; g.adj = d.adj; g.roots = d.roots; g.ok = root_ok; g.tree_bits = d.tree_bits;
+    g.emb = d.emb; g.bias = d.bias; g.d_emb = d_emb; g.d_bias = d_bias;
+    g.pi_in = v.pi_in; g.reach = v.reach; g.father = v.father;
+    g.items = rec.items; g.lev_off = rec.lev_off; g.n_lev = rec.n_lev;
+    g.kup = v.kup; g.kdn = v.kdn; g.big = v.big; g.big_cnt = v.big_cnt;
+    g.n_pairs = n_pairs; g.grad_emb = grad_emb; g.grad_bias = grad_bias;
+    {
+        int per_sm = 0;
+        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gg::reach_kernel, gg::GR_THREADS, 0));
+        GG_REQUIRE(per_sm >= 1, "expected G step reach kernel does not fit on an SM");
+        void *args[] = {(void *)&g};
+        GG_CHECK(cudaLaunchCooperativeKernel((const void *)gg::reach_kernel, dim3((unsigned)(gg::sm_count() * per_sm)),
+                                             dim3(gg::GR_THREADS), args, 0, st));
+    }
+    gg::score_kernel<<<(unsigned)(gg::sm_count() * 8), gg::GR_THREADS, 0, st>>>(g);
+    GG_CHECK(cudaGetLastError());
+    gg::npairs_kernel<<<(unsigned)(d.n_roots < gg::sm_count() * 4 ? d.n_roots : gg::sm_count() * 4), gg::GR_THREADS, 0, st>>>(g);
+    GG_CHECK(cudaGetLastError());
+    gg::big_nodes_kernel<<<(unsigned)((d.n_node + 255) / 256), 256, 0, st>>>(g);
+    GG_CHECK(cudaGetLastError());
+    switch (d.ld / 32) {
+        case 1: return gg::launch_gather<1>(g, st);
+        case 2: return gg::launch_gather<2>(g, st);
+        case 4: return gg::launch_gather<4>(g, st);
+        case 8: return gg::launch_gather<8>(g, st);
+        default: return gg::launch_gather<16>(g, st);
+    }
+}

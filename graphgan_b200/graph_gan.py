@@ -162,6 +162,15 @@ class GraphGAN(object):
         g, d = self.generator, self.discriminator
         return self.sampler.game_value_grad_d(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
 
+    def expected_g_grad(self, roots):
+        """The exact expectation, per G-mode walk, of the reference's generator step over the window pairs of the walks
+        from ``roots`` (DESIGN.md section 5.6), with config.window_size and the current models: sampler.WalkSampler.
+        expected_g_grad.  Returns device (n_pairs fp64, root_ok int32, grad_emb fp64 [N, ld], grad_bias fp64 [N])."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        return self.sampler.expected_g_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots),
+                                            window=config.window_size)
+
     def _trees_of(self, roots):
         """the trees of ``roots``: rows of the resident trees when they hold every one of them, else built"""
         t = self.trees
@@ -194,7 +203,10 @@ class GraphGAN(object):
         over the ok roots of value_roots() (nan when there are none).  With config.value_grad, " gnorm:<norm>" follows:
         the 2-norm of the gradient of the mean V over (E_G[:, :n_emb], b_G), exact (game_value_grad).  With
         config.value_grad_d, " dnorm:<norm>" comes last: the same for the discriminator, over (E_D[:, :n_emb], b_D)
-        (game_value_grad_d)."""
+        (game_value_grad_d).  With config.value_gcos, " gcos:<cos>" follows them: the cosine over (E_G[:, :n_emb], b_G)
+        between the expectation of the reference's generator step (expected_g_grad) and the gradient of the sum of V
+        (game_value_grad; computed for it alone when value_grad is off).  A positive value means the reference's step, which
+        descends its own loss, descends V on average."""
         vg, vd = getattr(config, "value_grad", False), getattr(config, "value_grad_d", False)
         if vg:
             pos, neg, ok, g_emb, g_bias = self.game_value_grad(self.value_roots())
@@ -216,6 +228,15 @@ class GraphGAN(object):
         if vd:
             sq = float((d_emb[:, :self.discriminator.n_emb] ** 2).sum().item() + (d_bias ** 2).sum().item())
             line += " dnorm:%r" % (float(np.sqrt(sq) / n) if n else np.nan)
+        if getattr(config, "value_gcos", False):
+            if not vg:
+                g_emb, g_bias = self.game_value_grad(self.value_roots())[3:]
+            r_emb, r_bias = self.expected_g_grad(self.value_roots())[2:]
+            k = self.generator.n_emb
+            dot = float((r_emb[:, :k] * g_emb[:, :k]).sum().item() + (r_bias * g_bias).sum().item())
+            nr = float(np.sqrt((r_emb[:, :k] ** 2).sum().item() + (r_bias ** 2).sum().item()))
+            ng = float(np.sqrt((g_emb[:, :k] ** 2).sum().item() + (g_bias ** 2).sum().item()))
+            line += " gcos:%r" % (dot / (nr * ng) if nr > 0 and ng > 0 else np.nan)
         return line + "\n"
 
     # ------------------------------------------------------------------ training on the exact game (DESIGN.md section 5.5)

@@ -533,6 +533,54 @@ class WalkSampler:
         pos[order], neg[order], ok[order] = sp, sn, so
         return pos, neg, ok, grad_emb, grad_bias
 
+    # ------------------------------------------------------------------ expected reference G step
+    def expected_g_grad(self, g_emb, g_bias, d_emb, d_bias, trees, *, window, max_scratch_bytes=None, reuse=None):
+        """The exact expectation, per G-mode walk, of the reference's generator step (csrc/value_gref.cu, DESIGN.md section
+        5.6): the window pairs of the walk's body (graph_gan.py:272-291, ``window`` = config.window_size, 1 .. 8), each
+        weighted by D's reward and differentiated as generator.py:22-31 does, with the sampled pairs held fixed.  The law is
+        ``distribution``'s (current father-removal bits); lambda_gen and the 1 / batch mean are not included.
+        Returns device (n_pairs fp64 [R]: the expected pairs per walk, root_ok int32 [R]) in the order of ``trees``, and
+        (grad_emb fp64 [N, ld], grad_bias fp64 [N]) for the padded rows ``g_emb`` (pad columns exactly 0) and ``g_bias``.
+        The roots are taken in ascending id order (stable for duplicates), in chunks under the budget rule of
+        ``distribution`` (``max_scratch_bytes``, default 2 GiB or env GG_GDIST_SCRATCH), each coordinate one fp64 chain
+        over the roots: the bits do not depend on the chunking, the order of the roots or the call."""
+        window = int(window)
+        if not 1 <= window <= 8:
+            raise ValueError("window must be 1 .. 8, got %d" % window)
+        torch, g = self.torch, self.g
+        assert g_emb.dtype == torch.float32 and g_emb.is_contiguous() and g_bias.dtype == torch.float32
+        assert d_emb.dtype == torch.float32 and d_emb.is_contiguous() and d_bias.dtype == torch.float32
+        assert d_emb.shape == g_emb.shape and int(d_bias.shape[0]) == g.n_node and int(g_emb.shape[0]) == g.n_node
+        R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
+        n_pairs = torch.zeros(R, dtype=torch.float64, device=self.device)
+        ok = torch.zeros(R, dtype=torch.int32, device=self.device)
+        grad_emb = torch.zeros(tuple(g_emb.shape), dtype=torch.float64, device=self.device)
+        grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
+        if R == 0:
+            return n_pairs, ok, grad_emb, grad_bias
+        order = torch.argsort(trees.roots.long(), stable=True)
+        st_trees = trees.select(order)
+        reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
+
+        def scratch_bytes(k):
+            nb = C.c_int64(0)
+            _cabi.check(self.lib.gg_expected_g_grad_scratch_bytes(N, nnz, k, window, C.byref(nb)),
+                        "gg_expected_g_grad_scratch_bytes")
+            return nb.value
+        chunk = max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
+        sn, so = torch.zeros_like(n_pairs), torch.zeros_like(ok)
+        d = self._law_desc(g_emb, g_bias, st_trees, reuse, None)
+        st = self._stream()
+        for lo in range(0, R, chunk):
+            hi = min(R, lo + chunk)
+            d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(st_trees.roots[lo:hi]), ptr(st_trees.tree_bits[lo:hi])
+            _cabi.check(self.lib.gg_expected_g_grad(C.byref(d), ptr(d_emb), ptr(d_bias), window, ptr(sn[lo:hi]), ptr(so[lo:hi]),
+                                                    ptr(grad_emb), ptr(grad_bias), ptr(scratch), scratch.numel(), st),
+                        "gg_expected_g_grad")
+        n_pairs[order], ok[order] = sn, so
+        return n_pairs, ok, grad_emb, grad_bias
+
     def finalize(self, out):
         _cabi.check(self.lib.gg_walk_finalize(out.n_roots, ptr(out.walk_ptr), int(out.for_d), ptr(out.samples),
                                               ptr(out.status), ptr(out.first_edge), ptr(out.wsteps), ptr(out.wsuml),

@@ -28,7 +28,8 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 11  /* 11: gg_adam_apply_dense; 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
+#define GG_ABI_VERSION 11  /* 11: gg_adam_apply_dense, then gg_expected_g_grad (an addition: every older entry point keeps
+                              its signature and meaning, and _cabi.lib() refuses a library that lacks a declared symbol); 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
 
 /* walk status codes (per walk) */
 enum { GG_NOTRUN = 0, GG_DONE = 1, GG_VOID = 2, GG_SKIPPED = 3 };
@@ -230,6 +231,27 @@ int gg_game_value_grad_d(int64_t n_node, int32_t ld, const float *emb, const flo
                          const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist,
                          const int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes,
                          void *stream);
+
+/* The exact expectation of the reference's generator step (csrc/value_gref.cu, DESIGN.md section 5.6): for the roots of g
+ * (the generator's law as gg_generator_dist computes it from g's fields, G mode, current father-removal bits) and the
+ * discriminator d_emb / d_bias (g->ld columns), writes root_ok (device int32 [n_roots], the root_ok of gg_generator_dist)
+ * and n_pairs (device fp64 [n_roots]: the expected number of window pairs per walk, sum_y reach(y) 2 min(window, depth(y)),
+ * 0 where root_ok = 0), and ADDS the expected per-walk sum of the production pair gradients of the window pairs
+ * (graph_gan.py:204-223 and :272-291 with config.window_size = window, generator.py:22-31) into grad_emb (device fp64
+ * [n_node, ld]) and grad_bias (device fp64 [n_node]):
+ *   for every reached y != root, d = 1 .. min(window, depth(y)), x = anc_d(y), and both ordered pairs (n1, n2) of {x, y}:
+ *   grad_emb[n1] += rho kappa emb[n2],  grad_emb[n2] += rho kappa emb[n1],  grad_bias[n2] += rho kappa
+ * rho = reach(y), the probability that a walk passes y; kappa = the fp32 coefficient of gg_pair_grad mode 1 with batch_total
+ * 1 and the reward of gg_pair_reward as a_k (lambda_gen and the 1 / batch mean are not included).  The sampled pairs are
+ * held fixed: no term flows through the law.  Pad columns receive exactly 0.  window: 1 .. 8.  Each node's row takes the
+ * roots in the order given as one fp64 chain per coordinate, continued from the value already in grad_emb / grad_bias:
+ * pass the roots in ascending id order (and chunks in order) for bits that do not depend on the order or the chunking.
+ * scratch: device, at least gg_expected_g_grad_scratch_bytes(n_node, nnz, n_roots, window) bytes (host-only size
+ * computation; gg_generator_dist's plus 20 + 8 window bytes per (root, node)). */
+int gg_expected_g_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int32_t window, int64_t *bytes);
+int gg_expected_g_grad(const gg_walk_desc *g, const float *d_emb, const float *d_bias, int32_t window, double *n_pairs,
+                       int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes,
+                       void *stream);
 
 /* prepare_data_for_d's output rows (graph_gan.py:192-201): for every accepted root, in batch
  * order: [i]*k + [i]*k | pos + neg | 1*k + 0*k.  row_ptr: device [R+1] scratch/out (exclusive
