@@ -240,11 +240,15 @@ __global__ void __launch_bounds__(WARPS_PER_CTA * 32, walk_min_ctas(CPL)) step1_
         const int c = __ldg(d.adj + e);
         const bool inc_father = !d.for_d && !((d.d1_bits[e >> 5] >> (e & 31)) & 1u);   // graph_gan.py:258-259
         int n; float m; int *ids; float *sc;
-        build_list<CPL, UNR_S1>(d, tb, c, root, inc_father, s_ids, s_sc, g_ids, g_sc, lane, n, m, ids, sc, rows_gathered, cyc, stg);
+        // a list too long for the warp's shared id buffer is enumerated straight into its slice of the pool (degree + 1
+        // entries): no copy from the global scratch afterwards
+        build_list<CPL, UNR_S1>(d, tb, c, root, inc_father, s_ids, s_sc, d.s1_ids + __ldg(d.s1_ptr + pos), g_sc, lane, n, m, ids, sc,
+                                rows_gathered, cyc, stg);
         if (lane == 0) d.s1_n[pos] = n;
         if (n == 0) continue;
         const long long o = __ldg(d.s1_ptr + pos);
-        for (int i = lane; i < n; i += 32) d.s1_ids[o + i] = ids[i];
+        if (ids == s_ids)
+            for (int i = lane; i < n; i += 32) d.s1_ids[o + i] = ids[i];
         if (n > 1) cdf_store_raw<UNR_S1>(sc, n, m, d.s1_q + o, lane);
         __syncwarp();
     }

@@ -13,6 +13,7 @@ torch.profiler (CUDA activities only) for --passes passes and writes ONE JSON re
   stage       flat_start_kernel, the walk_kernel tail, and the whole walk stage (first to last of its kernels);
   precompute  device microseconds per pass of the per-pass precompute kernels (the hub score kernel and root_cdf_kernel),
               from a second profiled region of --passes whole passes of its own.
+  depth1      the same for the depth-1 stage (root_step_kernel, step1_cdf_kernel), from the same region.
 
 The levels reuse kernel names, so a kernel is given to a level by launch order within the pass.  Load an A/B library
 with GG_LIB=<path> (tools/variants.py) to profile another build.
@@ -81,12 +82,16 @@ def split_levels(events, n_passes):
     return passes
 
 
-def precompute_kernels(events, n_passes):
-    """{kernel: microseconds per pass} of the precompute kernels (hub_score*_kernel, root_cdf_kernel)"""
+DEPTH1_KERNELS = ("root_step_kernel", "step1_cdf_kernel")
+
+
+def precompute_kernels(events, n_passes, depth1=False):
+    """{kernel: microseconds per pass} of the precompute kernels (hub_score*_kernel, root_cdf_kernel), or with depth1 of
+    the depth-1 stage (root_step_kernel, step1_cdf_kernel)"""
     tot, cnt = {}, {}
     for _, dur, name in events:
         base = name.split("<")[0]
-        if base.startswith("hub_score") or base == "root_cdf_kernel":
+        if (base in DEPTH1_KERNELS) if depth1 else (base.startswith("hub_score") or base == "root_cdf_kernel"):
             tot[name] = tot.get(name, 0) + dur
             cnt[name] = cnt.get(name, 0) + 1
     for k, c in cnt.items():
@@ -162,6 +167,7 @@ def main():
             one_pass(3000 + s)
         torch.cuda.synchronize()
     pre = precompute_kernels(kernel_events(prof_pre), args.passes)
+    depth1 = precompute_kernels(kernel_events(prof_pre), args.passes, depth1=True)
     ctr =np.stack([c.view(torch.int32).cpu().numpy().astype(np.int64) for c in ctrs])   # [passes, words]
 
     levels = {}
@@ -186,6 +192,7 @@ def main():
         "walk_stage_span_us": round(float(np.mean([sp[1] - sp[0] for _, sp in passes])) / 1e3, 2),
         "walk_stage_kernel_sum_us": round(float(np.mean([sum(sum(v.values()) for v in per.values()) for per, _ in passes])) / 1e3, 2),
         "precompute_us": pre, "precompute_total_us": round(sum(pre.values()), 2),
+        "depth1_us": depth1, "depth1_total_us": round(sum(depth1.values()), 2),
         "hub_entries": int(dg.hub_tiles(smp.hub_threshold)[3]),
         "note":"device time per pass (mean over the profiled passes); span = first walk-stage kernel start to the tail's "
                 "end, kernel_sum = the sum of the stage's kernel durations (the gaps between them are the difference)",
