@@ -50,6 +50,7 @@ SIGNATURES = {
     "gg_walk_sample": (C.c_int, [C.POINTER(WalkDesc), _P]),
     "gg_generator_dist_scratch_bytes": (C.c_int, [_I64, _I64, _I64, C.POINTER(_I64)]),
     "gg_generator_dist": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _P, _I64, _P]),
+    "gg_generator_dist_d": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _P, _P, _I64, _P]),
     "gg_game_value_scratch_bytes": (C.c_int, [_I64, _I64, C.POINTER(_I64)]),
     "gg_game_value": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P, _P, _P, _P, _I64, _P]),
     "gg_game_value_grad_scratch_bytes": (C.c_int, [_I64, _I64, _I64, C.POINTER(_I64)]),
@@ -58,6 +59,8 @@ SIGNATURES = {
     "gg_game_value_grad_d": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P, _P, _P, _I64, _P]),
     "gg_expected_g_grad_scratch_bytes": (C.c_int, [_I64, _I64, _I64, _I32, C.POINTER(_I64)]),
     "gg_expected_g_grad": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _I32, _P, _P, _P, _P, _P, _I64, _P]),
+    "gg_expected_d_grad_scratch_bytes": (C.c_int, [_I64, _I32, _I64, C.POINTER(_I64)]),
+    "gg_expected_d_grad": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P]),
     "gg_walk_finalize": (C.c_int, [_I64, _P, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "gg_emit_d_rows": (C.c_int, [_I64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "gg_bfs_scratch_bytes": (C.c_int, [_I64, _I64, C.POINTER(_I64)]),

@@ -62,6 +62,8 @@ value_grad = False                 # with value_roots > 0: the value line also e
 value_grad_d = False               # with value_roots > 0: the value line ends in " dnorm:<|grad_D mean V|_2>", exact (section 5.4)
 value_gcos = False                 # with value_roots > 0: the value line ends in " gcos:<cos>", the cosine between the exact
                                     # expectation of the reference's G step and grad_G V (DESIGN.md section 5.6)
+value_dcos = False                 # with value_roots > 0: the value line ends in " dcos:<cos>" (after gcos), the cosine
+                                    # between the exact expectation of the reference's D step and grad_D V (section 5.7)
 exact_roots = 0                     # > 0: train() plays the exact game on this many seeded roots (DESIGN.md section 5.5):
                                     # each D / G step is an Adam step on the exact gradient of the mean V; no walks are
                                     # sampled.  Single process only.  0: the reference's sampled training

@@ -58,11 +58,13 @@ size_t gdist_layout(void *buf, long long n_node, long long nnz_words, long long 
 
 // One item: the law of the walk's step from node it.y of root slot it.x.  REC: also record the step law of the item's
 // list per node (DESIGN.md section 5.3): pi_in of every reached child, pi_stop of the node, the child's father.
-template <int CPL, bool REC = false>
+// DM: the D-mode law (section 5.7): every depth-1 item goes without its father whatever d1_bits holds, and a depth-1
+// leaf adds its reach to p_void[slot] (the walk voids the root's pass) instead of voiding the row.
+template <int CPL, bool REC = false, bool DM = false>
 __device__ __forceinline__ void gdist_item(const gg_walk_desc &d, double *__restrict__ dist, int *__restrict__ root_ok,
                                            const GdView &v, const int4 it, int4 *out, unsigned *out_cnt, int *s_ids,
                                            float *s_sc, int lane, unsigned long long &rows, unsigned int (&cyc)[7],
-                                           Stage &stg, const GdRec &rec = GdRec()) {
+                                           Stage &stg, const GdRec &rec = GdRec(), double *p_void = nullptr) {
     const int slot = it.x, a = it.y, fa = it.z;
     const bool is_root = fa < 0, removed = it.w != 0;
     const bool inc_father = !is_root && !removed;           // graph_gan.py:250-259, G mode (d1 bits: :258-259)
@@ -80,6 +82,15 @@ __device__ __forceinline__ void gdist_item(const gg_walk_desc &d, double *__rest
     if (n == 0) {
         // a root without children voids every walk (graph_gan.py:252-253): root_ok stays 0.  Elsewhere only a node whose
         // father entry was removed can have an empty list (a D pass never leaves one): walks reaching it void the root.
+        if constexpr (DM) {
+            // D mode: only a depth-1 leaf has an empty list (graph_gan.py:255-257); its reach is the root's void mass,
+            // a multiple of 2^-53 whose sum is exact in any order
+            if (lane == 0 && !is_root) {
+                atomicAdd(p_void + slot, reach);
+                row[a] = 0.0;
+            }
+            return;
+        }
         if (lane == 0 && !is_root) {
             row[a] = 0.0;
             root_ok[slot] = -1;                              // (row cleared at the end of the launch)
@@ -136,7 +147,8 @@ __device__ __forceinline__ void gdist_item(const gg_walk_desc &d, double *__rest
         if (e < a1 && ((__ldg(tb + (e >> 5)) >> (e & 31)) & 1u)) {
             child = __ldg(d.adj + e);
             take = row[child] > 0.0;
-            rm = d.d1_bits ? (int)((__ldg(d.d1_bits + (e >> 5)) >> (e & 31)) & 1u) : 0;
+            if constexpr (DM) rm = 1;                        // graph_gan.py:258-259: D mode always removes the root
+            else rm = d.d1_bits ? (int)((__ldg(d.d1_bits + (e >> 5)) >> (e & 31)) & 1u) : 0;
         }
         warp_append(take, out, out_cnt, make_int4(slot, child, a, rm), lane);
     }
@@ -176,6 +188,40 @@ gdist_kernel(const __grid_constant__ gg_walk_desc d, double *__restrict__ dist, 
         for (long long i = threadIdx.x; i < d.n_node; i += blockDim.x) row[i] = 0.0;
         __syncthreads();
         if (threadIdx.x == 0) root_ok[k] = 0;
+    }
+    if (lane == 0 && rows && d.counters) atomicAdd(d.counters + GG_CNT_ROWS_GATHERED, rows);
+}
+
+// The D-mode law (DESIGN.md section 5.7): gdist_kernel's levels with the D-mode item; p_void[slot] collects the reach of
+// the depth-1 leaves.  No root voids its row, so root_ok ends 1 (the root has children) or 0.
+template <int CPL>
+__global__ void __launch_bounds__(WARPS_PER_CTA * 32, walk_min_ctas(CPL))
+gdist_d_kernel(const __grid_constant__ gg_walk_desc d, double *__restrict__ dist, int *__restrict__ root_ok,
+               double *__restrict__ p_void, const GdView v) {
+    extern __shared__ __align__(16) unsigned char walk_smem[];
+    cg::grid_group grid = cg::this_grid();
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    float *s_sc = reinterpret_cast<float *>(walk_smem + (size_t)wid * WALK_SMEM_PER_WARP);
+    int *s_ids = reinterpret_cast<int *>(s_sc + SC_CAP);
+    Stage stg;
+    stg.buf = s_sc; stg.bar = nullptr; stg.phase = 0u; stg.on = false;
+    const long long gw = (long long)blockIdx.x * WARPS_PER_CTA + wid, nw = (long long)gridDim.x * WARPS_PER_CTA;
+    const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+    unsigned long long rows = 0;
+    unsigned int cyc[7] = {0, 0, 0, 0, 0, 0, 0};
+    for (long long k = tid; k < d.n_roots; k += nt) v.list[0][k] = make_int4((int)k, __ldg(d.roots + k), -1, 0);
+    if (tid == 0) v.cnt[0] = (unsigned)d.n_roots;
+    grid.sync();
+    for (int lev = 0;; ++lev) {
+        const unsigned n_items = *(volatile unsigned *)(v.cnt + lev % 3);
+        if (n_items == 0) break;
+        if (tid == 0) v.cnt[(lev + 2) % 3] = 0;
+        const int4 *in = v.list[lev & 1];
+        int4 *out = v.list[(lev + 1) & 1];
+        for (long long i = gw; i < (long long)n_items; i += nw)
+            gdist_item<CPL, false, true>(d, dist, root_ok, v, in[i], out, v.cnt + (lev + 1) % 3, s_ids, s_sc, lane, rows,
+                                         cyc, stg, GdRec(), p_void);
+        grid.sync();
     }
     if (lane == 0 && rows && d.counters) atomicAdd(d.counters + GG_CNT_ROWS_GATHERED, rows);
 }
@@ -334,5 +380,38 @@ extern "C" int gg_generator_dist(const gg_walk_desc *dp, double *dist, int32_t *
     double *dist_p = dist;
     int *ok_p = root_ok;
     void *args[] = {(void *)&d, (void *)&dist_p, (void *)&ok_p, (void *)&v};
+    return gg::launch_gdist(kern, d, args, st);
+}
+
+extern "C" int gg_generator_dist_d(const gg_walk_desc *dp, double *dist, double *p_void, int32_t *root_ok, void *scratch,
+                                   int64_t scratch_bytes, void *stream) {
+    GG_REQUIRE(dp, "null descriptor");
+    const gg_walk_desc &d = *dp;
+    GG_REQUIRE(gg::ld_supported(d.ld), GG_LD_MESSAGE);
+    if (d.n_roots == 0) return 0;
+    GG_REQUIRE(d.n_node > 0 && d.emb && d.bias && d.indptr && d.adj && d.roots && d.tree_bits, "null graph/embedding pointer");
+    GG_REQUIRE(d.tree_words > 0, "tree_words missing (gg_tree_words)");
+    GG_REQUIRE(dist && p_void && root_ok && scratch, "null output or scratch pointer");
+    GG_REQUIRE(d.n_roots * d.n_node < (1ll << 31), "n_roots * n_node must be below 2^31 (process the roots in chunks)");
+    GG_REQUIRE(!d.edge_score || (d.hub_threshold > 0 && d.hub_threshold < gg::SMEM_CAP), "hub_threshold out of range");
+    gg::GdView v;
+    const size_t need = gg::gdist_layout(scratch, d.n_node, d.tree_words - 1, d.n_roots, &v);
+    GG_REQUIRE(scratch_bytes >= (int64_t)need, "scratch too small (gg_generator_dist_scratch_bytes)");
+    cudaStream_t st = (cudaStream_t)stream;
+    GG_CHECK(cudaMemsetAsync(dist, 0, sizeof(double) * (size_t)d.n_roots * (size_t)d.n_node, st));
+    GG_CHECK(cudaMemsetAsync(p_void, 0, sizeof(double) * (size_t)d.n_roots, st));
+    GG_CHECK(cudaMemsetAsync(root_ok, 0, sizeof(int32_t) * (size_t)d.n_roots, st));
+    GG_CHECK(cudaMemsetAsync(v.cnt, 0, 3 * sizeof(unsigned), st));
+    const void *kern;
+    switch (d.ld / 32) {
+        case 1: kern = (const void *)gg::gdist_d_kernel<1>; break;
+        case 2: kern = (const void *)gg::gdist_d_kernel<2>; break;
+        case 4: kern = (const void *)gg::gdist_d_kernel<4>; break;
+        case 8: kern = (const void *)gg::gdist_d_kernel<8>; break;
+        default: kern = (const void *)gg::gdist_d_kernel<16>; break;
+    }
+    double *dist_p = dist, *pv_p = p_void;
+    int *ok_p = root_ok;
+    void *args[] = {(void *)&d, (void *)&dist_p, (void *)&ok_p, (void *)&pv_p, (void *)&v};
     return gg::launch_gdist(kern, d, args, st);
 }

@@ -131,28 +131,35 @@ __device__ __forceinline__ double dgrad_w(int m, double deg, double G, float s) 
     return __dsub_rn(pos, G != 0.0 ? __dmul_rn(G, sp) : 0.0);
 }
 
-enum class NegOut { Chain, H, W };
+enum class NegOut { Chain, H, W, WRef };
 
 // The tile partials of neg for root tile rt (roots rt * RT ..) and node tile t; the root rows are in s_root.  OUT = H: each
 // product h[k, v] = dist[k, v] * bce(s(c_k, v), 0) is stored instead of added (the value gradient, DESIGN.md section 5.3).
 // OUT = W: h[k, v] = dgrad_w of the multiplicity mult[k, v] and dist[k, v] is stored, 0 for roots with ok_k = 0 (the
-// discriminator gradient, section 5.4).
+// discriminator gradient, section 5.4).  OUT = WRef: dist holds the D-mode law P_D and h[k, v] = fl(a_k dgrad_w(mult,
+// deg, Q, s)) with Q = P_D / (1 - p_void[k]) and a_k = fl(deg accept[k]) (the expected reference D step, section 5.7).
 template <int CPL, NegOut OUT = NegOut::Chain>
 __device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_root, double *s_part, double *h = nullptr,
-                         const int *mult = nullptr) {
+                         const int *mult = nullptr, const double *p_void = nullptr, const double *accept = nullptr) {
     constexpr int LD = 32 * CPL, RT = val_root_tile(CPL), RJ = RT / 8;
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, g = lane & 7, grp = threadIdx.x >> 3;
     const long long k0 = (long long)rt * RT;
     double acc[RJ];
 #pragma unroll
     for (int j = 0; j < RJ; ++j) acc[j] = 0.0;
-    double rdeg[OUT == NegOut::W ? RJ : 1];           // W: |graph[c_k]| of lane g's roots, 0 when ok_k = 0
-    if constexpr (OUT == NegOut::W) {
+    constexpr bool WW = OUT == NegOut::W || OUT == NegOut::WRef;
+    double rdeg[WW ? RJ : 1];                        // W: |graph[c_k]| of lane g's roots, 0 when ok_k = 0
+    double rq[OUT == NegOut::WRef ? RJ : 1], ra[OUT == NegOut::WRef ? RJ : 1];   // WRef: 1 - p_void, a_k
+    if constexpr (WW) {
 #pragma unroll
         for (int j = 0; j < RJ; ++j) {
             const long long k = k0 + 8 * j + g;
             long long lo, deg;
             rdeg[j] = (k < a.n_roots && value_ok(a, k, lo, deg)) ? (double)deg : 0.0;
+            if constexpr (OUT == NegOut::WRef) {
+                rq[j] = rdeg[j] > 0.0 ? __dsub_rn(1.0, __ldg(p_void + k)) : 1.0;
+                ra[j] = rdeg[j] > 0.0 ? __dmul_rn(rdeg[j], __ldg(accept + k)) : 0.0;
+            }
         }
     }
     for (int i = 0; i < VAL_NPG; ++i) {
@@ -190,6 +197,13 @@ __device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_r
                 if (valid && k < a.n_roots) {
                     const size_t o = (size_t)k * (size_t)a.n_node + (size_t)v;
                     h[o] = rdeg[j] > 0.0 ? dgrad_w(__ldg(mult + o), rdeg[j], w[j], sc) : 0.0;
+                }
+            } else if constexpr (OUT == NegOut::WRef) {
+                const long long k = k0 + 8 * j + g;
+                if (valid && k < a.n_roots) {
+                    const size_t o = (size_t)k * (size_t)a.n_node + (size_t)v;
+                    const double q = w[j] != 0.0 ? __ddiv_rn(w[j], rq[j]) : 0.0;
+                    h[o] = rdeg[j] > 0.0 ? __dmul_rn(ra[j], dgrad_w(__ldg(mult + o), rdeg[j], q, sc)) : 0.0;
                 }
             } else {
                 if (w[j] != 0.0) acc[j] = __dadd_rn(acc[j], __dmul_rn(w[j], bce_logits(sc, false)));
@@ -296,6 +310,34 @@ __global__ void __launch_bounds__(VAL_THREADS) value_w_kernel(const ValArgs a, c
     }
 }
 
+// W_ref[k, v] for every (root, node) pair (DESIGN.md section 5.7): value_w_kernel with the D-mode law and the acceptance
+template <int CPL>
+__global__ void __launch_bounds__(VAL_THREADS) value_wref_kernel(const ValArgs a, const int *__restrict__ mult,
+                                                                 const double *__restrict__ p_void,
+                                                                 const double *__restrict__ accept, double *__restrict__ W) {
+    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
+    extern __shared__ __align__(16) unsigned char val_smem[];
+    float *s_root = reinterpret_cast<float *>(val_smem);
+    double *s_part = reinterpret_cast<double *>(val_smem + (size_t)RT * LD * sizeof(float));
+    const long long n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
+    long long cur_rt = -1;
+    for (long long item = blockIdx.x; item < n_items; item += gridDim.x) {
+        const long long rt = item / a.n_tiles, t = item % a.n_tiles;
+        if (rt != cur_rt) {
+            __syncthreads();
+            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
+                const long long k = rt * RT + i / (LD / 4);
+                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
+                reinterpret_cast<float4 *>(s_root)[i] = x;
+            }
+            __syncthreads();
+            cur_rt = rt;
+        }
+        neg_item<CPL, NegOut::WRef>(a, (int)rt, t, s_root, s_part, W, mult, p_void, accept);
+    }
+}
+
 // neg_c = -(sum of the root's tile partials); warp per root
 __global__ void __launch_bounds__(256) value_reduce_kernel(const ValArgs a, double *__restrict__ neg, int *__restrict__ ok) {
     const int lane = threadIdx.x & 31;
@@ -356,7 +398,37 @@ int launch_value_w(const ValArgs &a, const int *mult, double *W, cudaStream_t st
     return check_cuda(cudaGetLastError(), "game value W launch");
 }
 
+template <int CPL>
+int launch_value_wref(const ValArgs &a, const int *mult, const double *p_void, const double *accept, double *W,
+                      cudaStream_t st) {
+    const size_t smem = val_smem_bytes(CPL);
+    int per_sm = 0;
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_wref_kernel<CPL>, VAL_THREADS, smem));
+    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
+    const long long RT = val_root_tile(CPL), n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
+    long long grid = (long long)sm_count() * per_sm;
+    if (grid > n_items) grid = n_items;
+    value_wref_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a, mult, p_void, accept, W);
+    return check_cuda(cudaGetLastError(), "expected D step W launch");
+}
+
 }  // namespace
+
+int value_wref_launch(long long n_node, int ld, const float *emb, const float *bias, const long long *raw_indptr,
+                      long long n_roots, const int *roots, const double *dist_d, const double *p_void, const int *ok_ref,
+                      const double *accept, const int *mult, double *W, cudaStream_t st) {
+    if (n_roots == 0) return 0;
+    ValArgs a = {};
+    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = val_tiles(n_node);
+    a.emb = emb; a.bias = bias; a.raw_indptr = raw_indptr; a.roots = roots; a.dist = dist_d; a.root_ok = ok_ref;
+    switch (ld / 32) {
+        case 1: return launch_value_wref<1>(a, mult, p_void, accept, W, st);
+        case 2: return launch_value_wref<2>(a, mult, p_void, accept, W, st);
+        case 4: return launch_value_wref<4>(a, mult, p_void, accept, W, st);
+        case 8: return launch_value_wref<8>(a, mult, p_void, accept, W, st);
+        default: return launch_value_wref<16>(a, mult, p_void, accept, W, st);
+    }
+}
 
 int value_w_launch(long long n_node, int ld, const float *emb, const float *bias, const long long *raw_indptr,
                    long long n_roots, const int *roots, const double *dist, const int *root_ok, const int *mult, double *W,

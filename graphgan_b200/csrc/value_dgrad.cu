@@ -14,6 +14,9 @@
 // them by id) as one fp64 chain continued from the caller's accumulator; per root k with ok_k = 1:
 //   acc = fma(W[k, r], E_D[c_k][i], acc) when W[k, r] != 0,  then acc = acc + C_k[i] when c_k = r;
 // the bias chain is accb = accb + W[k, r] when W[k, r] != 0.
+//
+// The expected reference D step of one pass (gg_expected_d_grad, DESIGN.md section 5.7) runs the same passes with
+// W_ref (value.cu's WRef store) in place of W and ok_ref in place of ok, after accept_kernel has formed P_acc and ok_ref.
 #include "value_grad.cuh"
 
 namespace gg {
@@ -179,6 +182,29 @@ __global__ void __launch_bounds__(DG_THREADS) node_kernel(const DgArgs a) {
     }
 }
 
+// P_acc = (1 - p_void)^deg_c by square-and-multiply from the least significant bit of deg_c, one __dmul_rn per step;
+// ok_ref = deg_c > 0, the root has children (root_ok = 1) and P_acc > 0.  accept is 0 where ok_ref is 0.
+__global__ void __launch_bounds__(256) accept_kernel(long long n_roots, const long long *__restrict__ raw_indptr,
+                                                     const int *__restrict__ roots, const double *__restrict__ p_void,
+                                                     const int *__restrict__ root_ok, double *__restrict__ accept,
+                                                     int *__restrict__ ok_ref) {
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_roots) return;
+    const int c = __ldg(roots + k);
+    long long e = __ldg(raw_indptr + c + 1) - __ldg(raw_indptr + c);
+    double p = 0.0;
+    if (e > 0 && __ldg(root_ok + k) == 1) {
+        double base = __dsub_rn(1.0, __ldg(p_void + k));
+        p = 1.0;
+        for (; e > 0; e >>= 1) {
+            if (e & 1) p = __dmul_rn(p, base);
+            base = __dmul_rn(base, base);
+        }
+    }
+    accept[k] = p;
+    ok_ref[k] = p > 0.0 ? 1 : 0;
+}
+
 template <int CPL>
 int launch_passes(const DgArgs &a, cudaStream_t st) {
     {
@@ -228,6 +254,13 @@ size_t dg_layout(void *buf, long long n_node, int ld, long long n_roots, DgLayou
     return off;
 }
 
+// gg_expected_d_grad's scratch: dg_layout, then ok_ref [n_roots]
+size_t dref_layout(void *buf, long long n_node, int ld, long long n_roots, DgLayout *v, int **ok_ref) {
+    const size_t off = dg_layout(buf, n_node, ld, n_roots, v);
+    if (buf && ok_ref) *ok_ref = reinterpret_cast<int *>(static_cast<unsigned char *>(buf) + off);
+    return off + (((size_t)n_roots * sizeof(int) + 255) & ~(size_t)255);
+}
+
 }  // namespace
 }  // namespace gg
 
@@ -261,6 +294,50 @@ extern "C" int gg_game_value_grad_d(int64_t n_node, int32_t ld, const float *emb
     gg::mult_kernel<<<(unsigned)n_roots, gg::DG_THREADS, 0, st>>>(a);
     GG_CHECK(cudaGetLastError());
     int rc = gg::value_w_launch(n_node, ld, emb, bias, a.raw_indptr, n_roots, roots, dist, root_ok, v.mult, v.W, st);
+    if (rc) return rc;
+    switch (ld / 32) {
+        case 1: return gg::launch_passes<1>(a, st);
+        case 2: return gg::launch_passes<2>(a, st);
+        case 4: return gg::launch_passes<4>(a, st);
+        case 8: return gg::launch_passes<8>(a, st);
+        default: return gg::launch_passes<16>(a, st);
+    }
+}
+
+extern "C" int gg_expected_d_grad_scratch_bytes(int64_t n_node, int32_t ld, int64_t n_roots, int64_t *bytes) {
+    GG_REQUIRE(bytes && n_node >= 0 && n_roots >= 0, "bad arguments");
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
+    *bytes = (int64_t)gg::dref_layout(nullptr, n_node, ld, n_roots, nullptr, nullptr);
+    return 0;
+}
+
+extern "C" int gg_expected_d_grad(int64_t n_node, int32_t ld, const float *emb, const float *bias, const int64_t *raw_indptr,
+                                  const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist_d,
+                                  const double *p_void, const int32_t *root_ok, double *accept, double *grad_emb,
+                                  double *grad_bias, void *scratch, int64_t scratch_bytes, void *stream) {
+    GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
+    GG_REQUIRE(n_node > 0 && n_node < (1ll << 31), "n_node must lie in [1, 2^31)");
+    GG_REQUIRE(n_roots >= 0, "n_roots must be >= 0");
+    if (n_roots == 0) return 0;
+    GG_REQUIRE(emb && bias && raw_indptr && raw_adj && roots, "null graph/embedding pointer");
+    GG_REQUIRE(dist_d && p_void && root_ok, "null D-mode law pointer");
+    GG_REQUIRE(accept && grad_emb && grad_bias && scratch, "null output or scratch pointer");
+    gg::DgLayout v;
+    int *ok_ref = nullptr;
+    const size_t need = gg::dref_layout(scratch, n_node, ld, n_roots, &v, &ok_ref);
+    GG_REQUIRE(scratch_bytes >= (int64_t)need, "scratch too small (gg_expected_d_grad_scratch_bytes)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const long long *rip = (const long long *)raw_indptr;
+    gg::accept_kernel<<<(unsigned)((n_roots + 255) / 256), 256, 0, st>>>(n_roots, rip, roots, p_void, root_ok, accept, ok_ref);
+    GG_CHECK(cudaGetLastError());
+    gg::DgArgs a;
+    a.n_node = n_node; a.n_roots = n_roots; a.n_ctiles = gg::cen_tiles(n_node);
+    a.emb = emb; a.raw_indptr = rip; a.raw_adj = raw_adj; a.roots = roots; a.root_ok = ok_ref;
+    a.mult = v.mult; a.W = v.W; a.partial = v.partial; a.C = v.C; a.grad_emb = grad_emb; a.grad_bias = grad_bias;
+    GG_CHECK(cudaMemsetAsync(v.mult, 0, (size_t)n_roots * (size_t)n_node * sizeof(int), st));
+    gg::mult_kernel<<<(unsigned)n_roots, gg::DG_THREADS, 0, st>>>(a);
+    GG_CHECK(cudaGetLastError());
+    int rc = gg::value_wref_launch(n_node, ld, emb, bias, rip, n_roots, roots, dist_d, p_void, ok_ref, accept, v.mult, v.W, st);
     if (rc) return rc;
     switch (ld / 32) {
         case 1: return gg::launch_passes<1>(a, st);

@@ -28,5 +28,10 @@ int value_h_launch(long long n_node, int ld, const float *emb, const float *bias
 int value_w_launch(long long n_node, int ld, const float *emb, const float *bias, const long long *raw_indptr,
                    long long n_roots, const int *roots, const double *dist, const int *root_ok, const int *mult, double *W,
                    cudaStream_t st);
+// W_ref[k, v] = fl(fl(|graph[c_k]| accept[k]) dgrad_w(mult, |graph[c_k]|, Q, s)), Q = dist_d[k, v] / (1 - p_void[k]):
+// the expected reference D step per (root, node) (value_dgrad.cu, DESIGN.md section 5.7), 0 for roots with ok_ref = 0
+int value_wref_launch(long long n_node, int ld, const float *emb, const float *bias, const long long *raw_indptr,
+                      long long n_roots, const int *roots, const double *dist_d, const double *p_void, const int *ok_ref,
+                      const double *accept, const int *mult, double *W, cudaStream_t st);
 
 }  // namespace gg

@@ -171,6 +171,14 @@ class GraphGAN(object):
         return self.sampler.expected_g_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots),
                                             window=config.window_size)
 
+    def expected_d_grad(self, roots):
+        """The exact expectation of the reference's discriminator step of one pass over ``roots`` (DESIGN.md section 5.7),
+        with the current models: sampler.WalkSampler.expected_d_grad.  Returns device (accept fp64, p_void fp64, ok_ref
+        int32, grad_emb fp64 [N, ld], grad_bias fp64 [N])."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        return self.sampler.expected_d_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
+
     def _trees_of(self, roots):
         """the trees of ``roots``: rows of the resident trees when they hold every one of them, else built"""
         t = self.trees
@@ -206,7 +214,10 @@ class GraphGAN(object):
         (game_value_grad_d).  With config.value_gcos, " gcos:<cos>" follows them: the cosine over (E_G[:, :n_emb], b_G)
         between the expectation of the reference's generator step (expected_g_grad) and the gradient of the sum of V
         (game_value_grad; computed for it alone when value_grad is off).  A positive value means the reference's step, which
-        descends its own loss, descends V on average."""
+        descends its own loss, descends V on average.  With config.value_dcos, " dcos:<cos>" comes last: the cosine over
+        (E_D[:, :n_emb], b_D) between the expectation of the reference's D step of one pass (expected_d_grad) and the
+        gradient of the sum of V (game_value_grad_d; computed for it alone when value_grad_d is off).  A positive value
+        means the reference's D step ascends V on average."""
         vg, vd = getattr(config, "value_grad", False), getattr(config, "value_grad_d", False)
         if vg:
             pos, neg, ok, g_emb, g_bias = self.game_value_grad(self.value_roots())
@@ -237,6 +248,15 @@ class GraphGAN(object):
             nr = float(np.sqrt((r_emb[:, :k] ** 2).sum().item() + (r_bias ** 2).sum().item()))
             ng = float(np.sqrt((g_emb[:, :k] ** 2).sum().item() + (g_bias ** 2).sum().item()))
             line += " gcos:%r" % (dot / (nr * ng) if nr > 0 and ng > 0 else np.nan)
+        if getattr(config, "value_dcos", False):
+            if not vd:
+                d_emb, d_bias = self.game_value_grad_d(self.value_roots())[3:]
+            r_emb, r_bias = self.expected_d_grad(self.value_roots())[3:]
+            k = self.discriminator.n_emb
+            dot = float((r_emb[:, :k] * d_emb[:, :k]).sum().item() + (r_bias * d_bias).sum().item())
+            nr = float(np.sqrt((r_emb[:, :k] ** 2).sum().item() + (r_bias ** 2).sum().item()))
+            nd = float(np.sqrt((d_emb[:, :k] ** 2).sum().item() + (d_bias ** 2).sum().item()))
+            line += " dcos:%r" % (dot / (nr * nd) if nr > 0 and nd > 0 else np.nan)
         return line + "\n"
 
     # ------------------------------------------------------------------ training on the exact game (DESIGN.md section 5.5)

@@ -317,6 +317,23 @@ class WalkSampler:
             pass
         return dist, root_ok
 
+    def d_distribution(self, emb, bias, trees, *, reuse=None, max_scratch_bytes=None):
+        """The D-mode walk law (csrc/gdist.cu, DESIGN.md section 5.7): for every root of ``trees``, P_D(v | root), the
+        exact probability that one D-mode walk (graph_gan.py:225-270, for_d=True) stops at v, and p_void, the probability
+        that it lands on a depth-1 leaf and so voids the root's D pass (graph_gan.py:255-257).  A D walk removes the root
+        from every depth-1 list whatever the father-removal bits hold, so the law does not depend on them, and the walks
+        of one root are independent draws from it.  Returns device fp64 ``P_D [R, N]``, fp64 ``p_void [R]`` and int32
+        ``root_ok [R]`` (1 iff the root has children; sum_v P_D = 1 - p_void then).  ``reuse`` and the chunking as for
+        ``distribution``."""
+        torch = self.torch
+        R, N = int(trees.roots.shape[0]), self.g.n_node
+        dist = torch.empty((R, N), dtype=torch.float64, device=self.device)
+        root_ok = torch.empty(R, dtype=torch.int32, device=self.device)
+        p_void = torch.empty(R, dtype=torch.float64, device=self.device)
+        for _ in self._distribution_chunks(emb, bias, trees, reuse, max_scratch_bytes, None, dist, root_ok, p_void=p_void):
+            pass
+        return dist, p_void, root_ok
+
     def _law_desc(self, emb, bias, trees, reuse, counters):
         """the descriptor of the generator's law for gg_generator_dist / gg_game_value_grad (the per-chunk fields n_roots,
         roots, tree_bits are the caller's); with ``reuse``, the hub scores are refreshed first"""
@@ -333,11 +350,13 @@ class WalkSampler:
         return d
 
     def _distribution_chunks(self, emb, bias, trees, reuse, max_scratch_bytes, counters, dist=None, root_ok=None,
-                             extra_bytes=None):
+                             extra_bytes=None, p_void=None, d_mode=False):
         """gg_generator_dist over the roots of ``trees`` in chunks whose scratch fits the budget; yields (lo, hi, dist rows,
         root_ok rows) per chunk.  The rows go to dist[lo:hi] / root_ok[lo:hi] when those are given, else to one chunk-sized
         buffer that the next chunk overwrites.  ``extra_bytes(k)``: the caller's own scratch for a chunk of k roots, counted
-        against the same budget (None: nothing)."""
+        against the same budget (None: nothing).  With ``d_mode`` (implied by ``p_void``), gg_generator_dist_d instead:
+        the D-mode law, and each chunk yields (lo, hi, dist rows, root_ok rows, p_void rows), the p_void rows going to
+        p_void[lo:hi] when given, else to a chunk-sized buffer."""
         torch, g = self.torch, self.g
         R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
         if R == 0:
@@ -359,12 +378,24 @@ class WalkSampler:
             rows = lambda lo, hi: (dist[:hi - lo], root_ok[:hi - lo])
         else:
             rows = lambda lo, hi: (dist[lo:hi], root_ok[lo:hi])
+        d_mode = d_mode or p_void is not None
+        if d_mode and p_void is None:
+            p_void = torch.empty(chunk, dtype=torch.float64, device=self.device)
+            pv_rows = lambda lo, hi: p_void[:hi - lo]
+        else:
+            pv_rows = lambda lo, hi: p_void[lo:hi]
         d = self._law_desc(emb, bias, trees, reuse, counters)
         st = self._stream()
         for lo in range(0, R, chunk):
             hi = min(R, lo + chunk)
             dr, okr = rows(lo, hi)
             d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(trees.roots[lo:hi]), ptr(trees.tree_bits[lo:hi])
+            if d_mode:
+                pvr = pv_rows(lo, hi)
+                _cabi.check(self.lib.gg_generator_dist_d(C.byref(d), ptr(dr), ptr(pvr), ptr(okr), ptr(scratch),
+                                                         scratch.numel(), st), "gg_generator_dist_d")
+                yield lo, hi, dr, okr, pvr
+                continue
             _cabi.check(self.lib.gg_generator_dist(C.byref(d), ptr(dr), ptr(okr), ptr(scratch), scratch.numel(), st),
                         "gg_generator_dist")
             yield lo, hi, dr, okr
@@ -580,6 +611,52 @@ class WalkSampler:
                         "gg_expected_g_grad")
         n_pairs[order], ok[order] = sn, so
         return n_pairs, ok, grad_emb, grad_bias
+
+    # ------------------------------------------------------------------ expected reference D step
+    def expected_d_grad(self, g_emb, g_bias, d_emb, d_bias, trees, *, max_scratch_bytes=None, reuse=None):
+        """The exact expectation of the reference's discriminator step of one pass (csrc/value_dgrad.cu, DESIGN.md section
+        5.7): E[-grad sum_rows bce] over the rows prepare_data_for_d (graph_gan.py:182-202) emits for each root c -- deg_c =
+        |graph[c]| label-1 pairs from the raw list and deg_c label-0 pairs from D-mode walks, all kept with probability
+        P_acc = (1 - p_void)^deg_c, the negatives then independent draws from Q = P_D / (1 - p_void) (``d_distribution``).
+        lambda_dis, the 1 / batch mean and update_ratio are not included; the law is conditional on the root being drawn.
+        The sign is the descent direction of the reference's D loss, so it compares directly with ``game_value_grad_d``.
+        Returns device (accept fp64 [R]: P_acc, 0 where ok_ref = 0; p_void fp64 [R]; ok_ref int32 [R]: 1 iff deg_c > 0,
+        the root has children and P_acc > 0) in the order of ``trees``, and (grad_emb fp64 [N, ld], grad_bias fp64 [N])
+        for the padded rows ``d_emb`` (pad columns exactly 0) and ``d_bias``.  The roots are taken in ascending id order
+        (stable for duplicates), in the chunks of ``d_distribution`` with this step's scratch counted against the same
+        budget (``max_scratch_bytes``, default 2 GiB or env GG_GDIST_SCRATCH), each coordinate one fp64 chain over the
+        roots: the bits do not depend on the chunking, the order of the roots or the call."""
+        torch, g = self.torch, self.g
+        assert g_emb.dtype == torch.float32 and g_emb.is_contiguous() and g_bias.dtype == torch.float32
+        assert d_emb.dtype == torch.float32 and d_emb.is_contiguous() and d_bias.dtype == torch.float32
+        assert int(d_emb.shape[0]) == g.n_node and int(d_bias.shape[0]) == g.n_node
+        R, N, ld = int(trees.roots.shape[0]), g.n_node, int(d_emb.shape[1])
+        accept = torch.zeros(R, dtype=torch.float64, device=self.device)
+        p_void = torch.zeros(R, dtype=torch.float64, device=self.device)
+        grad_emb = torch.zeros(tuple(d_emb.shape), dtype=torch.float64, device=self.device)
+        grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
+        if R == 0:
+            return accept, p_void, torch.zeros(0, dtype=torch.int32, device=self.device), grad_emb, grad_bias
+        order = torch.argsort(trees.roots.long(), stable=True)
+        st_trees = trees.select(order)
+
+        def grad_bytes(k):
+            nb = C.c_int64(0)
+            _cabi.check(self.lib.gg_expected_d_grad_scratch_bytes(N, ld, k, C.byref(nb)), "gg_expected_d_grad_scratch_bytes")
+            return nb.value
+        sa, sv = torch.zeros_like(accept), torch.zeros_like(p_void)
+        st, ds = self._stream(), None
+        for lo, hi, dist, root_ok, pv in self._distribution_chunks(g_emb, g_bias, st_trees, reuse, max_scratch_bytes, None,
+                                                                   extra_bytes=grad_bytes, d_mode=True):
+            if ds is None:                                              # the first chunk is the largest
+                ds = torch.empty(max(grad_bytes(hi - lo), 16), dtype=torch.uint8, device=self.device)
+            sv[lo:hi] = pv
+            _cabi.check(self.lib.gg_expected_d_grad(N, ld, ptr(d_emb), ptr(d_bias), ptr(g.raw_indptr), ptr(g.raw_adj),
+                                                    hi - lo, ptr(st_trees.roots[lo:hi]), ptr(dist), ptr(pv), ptr(root_ok),
+                                                    ptr(sa[lo:hi]), ptr(grad_emb), ptr(grad_bias), ptr(ds), ds.numel(), st),
+                        "gg_expected_d_grad")
+        accept[order], p_void[order] = sa, sv
+        return accept, p_void, (accept > 0).to(torch.int32), grad_emb, grad_bias
 
     def finalize(self, out):
         _cabi.check(self.lib.gg_walk_finalize(out.n_roots, ptr(out.walk_ptr), int(out.for_d), ptr(out.samples),

@@ -28,7 +28,8 @@
 extern "C" {
 #endif
 
-#define GG_ABI_VERSION 11  /* 11: gg_adam_apply_dense, then gg_expected_g_grad (an addition: every older entry point keeps
+#define GG_ABI_VERSION 11  /* 11: gg_adam_apply_dense, then gg_expected_g_grad, then gg_generator_dist_d and
+                              gg_expected_d_grad (additions: every older entry point keeps
                               its signature and meaning, and _cabi.lib() refuses a library that lacks a declared symbol); 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
 
 /* walk status codes (per walk) */
@@ -180,6 +181,16 @@ int gg_generator_dist_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots
 int gg_generator_dist(const gg_walk_desc *d, double *dist, int32_t *root_ok, void *scratch, int64_t scratch_bytes,
                       void *stream);
 
+/* The D-mode walk law (csrc/gdist.cu, DESIGN.md section 5.7): gg_generator_dist for the walks of a discriminator pass
+ * (graph_gan.py:225-270, for_d = 1).  The root's list is its children, every depth-1 node's list its children (the root
+ * is removed whatever d->d1_bits holds, so d1_bits is not read and may be NULL), a deeper node's list [father] +
+ * children.  dist[k, v] = reach(v) * pi_v(father(v)) for depth >= 2, 0 at the root and at depth 1.  p_void[k] (device
+ * fp64 [n_roots]) = the sum of reach(a) over the depth-1 leaves a: the probability that one D walk voids the root's pass
+ * (graph_gan.py:255-257); a sum of multiples of 2^-53 at most 1, exact in any order.  root_ok[k] = 1 iff the root has
+ * children.  Every other field, the scratch (gg_generator_dist_scratch_bytes) and the limits as for gg_generator_dist. */
+int gg_generator_dist_d(const gg_walk_desc *d, double *dist, double *p_void, int32_t *root_ok, void *scratch,
+                        int64_t scratch_bytes, void *stream);
+
 /* The GraphGAN game value per root, exactly (csrc/value.cu, DESIGN.md section 5.2; Wang et al., AAAI-18, Eq. 1):
  *   V_c = pos_c + neg_c,  pos_c = -(1 / |graph[c]|) sum_k bce(s(c, graph[c][k]), 1)  (raw CSR, entry order, duplicates and
  *   self-loops count),  neg_c = -sum_v dist[k, v] bce(s(c, v), 0)  (v with dist[k, v] = 0 contribute exactly 0),
@@ -231,6 +242,23 @@ int gg_game_value_grad_d(int64_t n_node, int32_t ld, const float *emb, const flo
                          const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist,
                          const int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes,
                          void *stream);
+
+/* The exact expectation of the reference's discriminator step of one pass (csrc/value_dgrad.cu, DESIGN.md section 5.7):
+ * for the roots and the D-mode law of gg_generator_dist_d (dist_d, p_void, root_ok) and the discriminator emb / bias
+ * (other arguments as for gg_game_value_grad_d), writes accept (device fp64 [n_roots]): P_acc = (1 - p_void)^deg_c,
+ * deg_c = |graph[c]|, by square-and-multiply from the least significant bit (one fp64 product per step), 0 unless
+ * deg_c > 0 and root_ok = 1; ok_ref = accept > 0.  ADDS the expectation of -grad sum_rows bce over the rows
+ * prepare_data_for_d emits for the root (deg_c positives from the raw list, deg_c negatives from Q = dist_d / (1 - p_void),
+ * emitted with probability P_acc) into grad_emb / grad_bias with the assembly of gg_game_value_grad_d, W replaced by
+ *   W_ref[k, v] = fl(fl(deg_c P_acc) dgrad_w(n_kv, deg_c, Q[k, v], s))   (dgrad_w: gg_game_value_grad_d's W per pair)
+ * for ok_ref = 1 only; lambda_dis, the 1 / batch mean and update_ratio are not included.  The same order contract as
+ * gg_game_value_grad_d.  scratch: device, at least gg_expected_d_grad_scratch_bytes(n_node, ld, n_roots) bytes (host-only
+ * size computation; gg_game_value_grad_d_scratch_bytes' plus 4 bytes per root).  Six launches and one memset. */
+int gg_expected_d_grad_scratch_bytes(int64_t n_node, int32_t ld, int64_t n_roots, int64_t *bytes);
+int gg_expected_d_grad(int64_t n_node, int32_t ld, const float *emb, const float *bias, const int64_t *raw_indptr,
+                       const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist_d,
+                       const double *p_void, const int32_t *root_ok, double *accept, double *grad_emb, double *grad_bias,
+                       void *scratch, int64_t scratch_bytes, void *stream);
 
 /* The exact expectation of the reference's generator step (csrc/value_gref.cu, DESIGN.md section 5.6): for the roots of g
  * (the generator's law as gg_generator_dist computes it from g's fields, G mode, current father-removal bits) and the
