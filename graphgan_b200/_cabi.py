@@ -61,6 +61,11 @@ SIGNATURES = {
     "gg_expected_g_grad": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _I32, _P, _P, _P, _P, _P, _I64, _P]),
     "gg_expected_d_grad_scratch_bytes": (C.c_int, [_I64, _I32, _I64, C.POINTER(_I64)]),
     "gg_expected_d_grad": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P]),
+    "gg_best_response_scratch_bytes": (C.c_int, [_I64, _I64, _I64, C.POINTER(_I64)]),
+    "gg_best_response": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _P, _P, _P, _P, _I64, _P]),
+    "gg_best_response_grad_scratch_bytes": (C.c_int, [_I64, _I64, _I64, C.POINTER(_I64)]),
+    "gg_best_response_grad": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P]),
+    "gg_best_response_spmm": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _P, _P, _P, _P]),
     "gg_walk_finalize": (C.c_int, [_I64, _P, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "gg_emit_d_rows": (C.c_int, [_I64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "gg_bfs_scratch_bytes": (C.c_int, [_I64, _I64, C.POINTER(_I64)]),

@@ -64,6 +64,9 @@ value_gcos = False                 # with value_roots > 0: the value line ends i
                                     # expectation of the reference's G step and grad_G V (DESIGN.md section 5.6)
 value_dcos = False                 # with value_roots > 0: the value line ends in " dcos:<cos>" (after gcos), the cosine
                                     # between the exact expectation of the reference's D step and grad_D V (section 5.7)
+value_jsd = False                  # with value_roots > 0: the value line ends in " jsd:<mean JSD> hit:<mean hit>" (after
+                                    # dcos): G's exact Jensen-Shannon divergence from the data and its mass on the true
+                                    # neighbours, from the top two levels of each tree (DESIGN.md section 5.8)
 exact_roots = 0                     # > 0: train() plays the exact game on this many seeded roots (DESIGN.md section 5.5):
                                     # each D / G step is an Adam step on the exact gradient of the mean V; no walks are
                                     # sampled.  Single process only.  0: the reference's sampled training

@@ -128,6 +128,20 @@ class DeviceGraph:
             self._rev = rev if int(missing.item()) == 0 else None
         return self._rev
 
+    def entry_mult(self):
+        """mult[e] = the number of times adj[e] occurs in the raw list graph[u] of the entry's row u: n_ca of the walk-CSR
+        entry e = (c -> a), duplicates counted (device int32 [nnz], cached; computed once per graph on the host, like the
+        walk CSR itself).  p_true(a | c) = mult[e] / |graph[c]| (DESIGN.md section 5.8)."""
+        import torch
+        if not hasattr(self, "_mult"):
+            h, n = self.host, self.n_node
+            key_raw = np.repeat(np.arange(n, dtype=np.int64), np.diff(h.raw_indptr)) * n + h.raw_adj
+            key = np.repeat(np.arange(n, dtype=np.int64), np.diff(h.indptr)) * n + h.adj
+            u, cnt = np.unique(key_raw, return_counts=True)
+            mult = cnt[np.searchsorted(u, key)].astype(np.int32) if key.shape[0] else np.zeros(0, np.int32)
+            self._mult = torch.from_numpy(np.concatenate([mult, np.zeros(1, np.int32)])).to(self.device)[:max(key.shape[0], 1)]
+        return self._mult
+
     def hub_tiles(self, threshold, item_cap=HUB_ITEM_CAP):
         """Work list of gg_hub_scores, target-major: the walk-CSR entries e = (u -> v) of the nodes u whose degree is
         >= threshold, stably sorted by target v, as pairs (u, e) (device int32 [n_entries, 2]), and the work items

@@ -179,6 +179,22 @@ class GraphGAN(object):
         g, d = self.generator, self.discriminator
         return self.sampler.expected_d_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots))
 
+    def best_response(self, roots):
+        """The game value against the best discriminator, vstar_c = max_D V_c(G, D) = 2 JSD(p_true(.|c) || G(.|c)) - log 4,
+        and G's mass on the true neighbours, for every root c of ``roots`` (DESIGN.md section 5.8), with the current
+        generator: sampler.WalkSampler.best_response.  Returns device (vstar fp64, hit fp64, ok int32)."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g = self.generator
+        return self.sampler.best_response(g.emb, g.bias_t, self._trees_of(roots))
+
+    def best_response_grad(self, roots):
+        """best_response(roots) and the exact gradient of sum_{ok c} vstar_c with respect to the generator's padded rows
+        and biases (DESIGN.md section 5.8): sampler.WalkSampler.best_response_grad.  Returns device (vstar, hit, ok,
+        grad_emb fp64 [N, ld], grad_bias fp64 [N])."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g = self.generator
+        return self.sampler.best_response_grad(g.emb, g.bias_t, self._trees_of(roots))
+
     def _trees_of(self, roots):
         """the trees of ``roots``: rows of the resident trees when they hold every one of them, else built"""
         t = self.trees
@@ -217,7 +233,9 @@ class GraphGAN(object):
         descends its own loss, descends V on average.  With config.value_dcos, " dcos:<cos>" comes last: the cosine over
         (E_D[:, :n_emb], b_D) between the expectation of the reference's D step of one pass (expected_d_grad) and the
         gradient of the sum of V (game_value_grad_d; computed for it alone when value_grad_d is off).  A positive value
-        means the reference's D step ascends V on average."""
+        means the reference's D step ascends V on average.  With config.value_jsd, " jsd:<mean JSD> hit:<mean hit>" comes
+        last: the Jensen-Shannon divergence of the generator from the data and the generator's mass on the true
+        neighbours (best_response), means over the roots whose best-response ok is 1."""
         vg, vd = getattr(config, "value_grad", False), getattr(config, "value_grad_d", False)
         if vg:
             pos, neg, ok, g_emb, g_bias = self.game_value_grad(self.value_roots())
@@ -257,6 +275,12 @@ class GraphGAN(object):
             nr = float(np.sqrt((r_emb[:, :k] ** 2).sum().item() + (r_bias ** 2).sum().item()))
             nd = float(np.sqrt((d_emb[:, :k] ** 2).sum().item() + (d_bias ** 2).sum().item()))
             line += " dcos:%r" % (dot / (nr * nd) if nr > 0 and nd > 0 else np.nan)
+        if getattr(config, "value_jsd", False):
+            vs, ht, okb = (x.cpu().numpy() for x in self.best_response(self.value_roots()))
+            sb = okb == 1
+            nb = int(sb.sum())
+            jsd = float((vs[sb] / 2 + np.log(2.0)).mean()) if nb else np.nan
+            line += " jsd:%r hit:%r" % (jsd, float(ht[sb].mean()) if nb else np.nan)
         return line + "\n"
 
     # ------------------------------------------------------------------ training on the exact game (DESIGN.md section 5.5)
@@ -303,6 +327,20 @@ class GraphGAN(object):
         if n_ok:
             g.apply_dense_grad(gE, gb, 1.0 / n_ok)
         return pos, neg, ok
+
+    def exact_jsd_step(self, roots, *, max_scratch_bytes=None):
+        """One Adam step of the generator on the exact gradient of the mean Jensen-Shannon divergence JSD_c = vstar_c / 2
+        + log 2 over the ok roots of ``roots`` (DESIGN.md section 5.8): best_response_grad, then apply_dense_grad with
+        scale +1/(2 n_ok) (the L2 term is the model's own, as in exact_g_step).  A step without ok roots changes nothing.
+        Returns the pre-step device (vstar, hit, ok)."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g = self.generator
+        vstar, hit, ok, gE, gb = self.sampler.best_response_grad(g.emb, g.bias_t, self._exact_trees(roots),
+                                                                 max_scratch_bytes=max_scratch_bytes)
+        n_ok = int(ok.sum().item())
+        if n_ok:
+            g.apply_dense_grad(gE, gb, 1.0 / (2 * n_ok))
+        return vstar, hit, ok
 
     def exact_d_phase(self, roots, steps, *, max_scratch_bytes=None):
         """``steps`` exact D steps.  G is fixed meanwhile, so its law over the roots is computed once when it fits the

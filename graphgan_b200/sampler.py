@@ -658,6 +658,92 @@ class WalkSampler:
         accept[order], p_void[order] = sa, sv
         return accept, p_void, (accept > 0).to(torch.int32), grad_emb, grad_bias
 
+    # ------------------------------------------------------------------ the value against the best discriminator
+    def _best_response_chunks(self, g_emb, g_bias, trees, max_scratch_bytes, reuse, grad):
+        """(order, sorted trees, chunk size, scratch, descriptor) of best_response / best_response_grad"""
+        torch, g = self.torch, self.g
+        assert g_emb.dtype == torch.float32 and g_emb.is_contiguous() and g_bias.dtype == torch.float32
+        assert int(g_emb.shape[0]) == g.n_node and int(g_bias.shape[0]) == g.n_node
+        R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
+        order = torch.argsort(trees.roots.long(), stable=True)
+        ident = bool(torch.equal(order, torch.arange(R, device=order.device)))
+        st_trees = trees if ident else trees.select(order)             # (rows of nnz / 8 bytes: no copy when sorted)
+        reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
+        fn = self.lib.gg_best_response_grad_scratch_bytes if grad else self.lib.gg_best_response_scratch_bytes
+
+        def scratch_bytes(k):
+            nb = C.c_int64(0)
+            _cabi.check(fn(N, nnz, k, C.byref(nb)), "gg_best_response_scratch_bytes")
+            return nb.value
+        chunk = max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
+        return order, st_trees, chunk, scratch, self._law_desc(g_emb, g_bias, st_trees, reuse, None)
+
+    def best_response(self, g_emb, g_bias, trees, *, max_scratch_bytes=None, reuse=None):
+        """The game value against the best discriminator per root (csrc/best_response.cu, DESIGN.md section 5.8):
+        vstar_c = max_D V_c(G, D) = 2 JSD(p_true(.|c) || G(.|c)) - log 4, with p_true(a | c) = n_ca / |graph[c]| over the
+        raw list and G the generator's exact G-mode law (``distribution``, current father-removal bits) at c's neighbours,
+        which are the depth-1 nodes of c's tree: only the depth-1 lists are built.  hit_c = sum_a G(a | c), the
+        generator's mass on the true neighbours.  Returns device (vstar fp64 [R], hit fp64 [R], ok int32 [R]) in the order
+        of ``trees``; ok is ``game_value``'s (vstar = hit = 0 where ok = 0).  The roots are taken in ascending id order, in
+        chunks under the budget rule of ``distribution`` (``max_scratch_bytes``, default 2 GiB or env GG_GDIST_SCRATCH):
+        the bits do not depend on the chunking, the order of the roots or the call."""
+        torch, g = self.torch, self.g
+        R = int(trees.roots.shape[0])
+        vstar = torch.zeros(R, dtype=torch.float64, device=self.device)
+        hit = torch.zeros(R, dtype=torch.float64, device=self.device)
+        ok = torch.zeros(R, dtype=torch.int32, device=self.device)
+        if R == 0:
+            return vstar, hit, ok
+        order, st_trees, chunk, scratch, d = self._best_response_chunks(g_emb, g_bias, trees, max_scratch_bytes, reuse, False)
+        sv, sh, so = torch.zeros_like(vstar), torch.zeros_like(hit), torch.zeros_like(ok)
+        mult, st = g.entry_mult(), self._stream()
+        for lo in range(0, R, chunk):
+            hi = min(R, lo + chunk)
+            d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(st_trees.roots[lo:hi]), ptr(st_trees.tree_bits[lo:hi])
+            _cabi.check(self.lib.gg_best_response(C.byref(d), ptr(g.raw_indptr), ptr(mult), ptr(sv[lo:hi]), ptr(sh[lo:hi]),
+                                                  ptr(so[lo:hi]), ptr(scratch), scratch.numel(), st), "gg_best_response")
+        vstar[order], hit[order], ok[order] = sv, sh, so
+        return vstar, hit, ok
+
+    def best_response_grad(self, g_emb, g_bias, trees, *, max_scratch_bytes=None, reuse=None):
+        """``best_response`` and the exact gradient of sum_{ok c} vstar_c with respect to the generator's parameters
+        (DESIGN.md section 5.8): section 5.3's policy gradient with log(1 - D*) for D* = p / (p + G), held fixed (envelope
+        theorem).  Returns device (vstar fp64 [R], hit fp64 [R], ok int32 [R]) in the order of ``trees`` -- the bits of
+        ``best_response`` -- and (grad_emb fp64 [N, ld], grad_bias fp64 [N]) for the padded rows ``g_emb`` (pad columns
+        exactly 0) and ``g_bias``; lambda_gen is not included.  The roots are taken in ascending id order, in chunks under
+        the budget rule of ``distribution``; two fp64 accumulators per walk-CSR entry (16 bytes each) are held for the
+        whole call and turned into the gradient once at the end: the bits do not depend on the chunking, the order of the
+        roots or the call.  Needs a symmetric walk CSR (``DeviceGraph.reverse_entries``)."""
+        torch, g = self.torch, self.g
+        R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
+        vstar = torch.zeros(R, dtype=torch.float64, device=self.device)
+        hit = torch.zeros(R, dtype=torch.float64, device=self.device)
+        ok = torch.zeros(R, dtype=torch.int32, device=self.device)
+        grad_emb = torch.zeros(tuple(g_emb.shape), dtype=torch.float64, device=self.device)
+        grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
+        if R == 0:
+            return vstar, hit, ok, grad_emb, grad_bias
+        rev = g.reverse_entries()
+        if rev is None:
+            raise ValueError("best_response_grad needs a symmetric walk CSR (every entry has a reverse entry)")
+        order, st_trees, chunk, scratch, d = self._best_response_chunks(g_emb, g_bias, trees, max_scratch_bytes, reuse, True)
+        sv, sh, so = torch.zeros_like(vstar), torch.zeros_like(hit), torch.zeros_like(ok)
+        acc_coef = torch.zeros(max(nnz, 1), dtype=torch.float64, device=self.device)
+        acc_bias = torch.zeros(max(nnz, 1), dtype=torch.float64, device=self.device)
+        mult, st = g.entry_mult(), self._stream()
+        for lo in range(0, R, chunk):
+            hi = min(R, lo + chunk)
+            d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(st_trees.roots[lo:hi]), ptr(st_trees.tree_bits[lo:hi])
+            _cabi.check(self.lib.gg_best_response_grad(C.byref(d), ptr(g.raw_indptr), ptr(mult), ptr(rev), ptr(sv[lo:hi]),
+                                                       ptr(sh[lo:hi]), ptr(so[lo:hi]), ptr(acc_coef), ptr(acc_bias),
+                                                       ptr(scratch), scratch.numel(), st), "gg_best_response_grad")
+        _cabi.check(self.lib.gg_best_response_spmm(N, int(g_emb.shape[1]), ptr(g.indptr), ptr(g.adj), ptr(g_emb),
+                                                   ptr(acc_coef), ptr(acc_bias), ptr(grad_emb), ptr(grad_bias), st),
+                    "gg_best_response_spmm")
+        vstar[order], hit[order], ok[order] = sv, sh, so
+        return vstar, hit, ok, grad_emb, grad_bias
+
     def finalize(self, out):
         _cabi.check(self.lib.gg_walk_finalize(out.n_roots, ptr(out.walk_ptr), int(out.for_d), ptr(out.samples),
                                               ptr(out.status), ptr(out.first_edge), ptr(out.wsteps), ptr(out.wsuml),

@@ -29,7 +29,8 @@ extern "C" {
 #endif
 
 #define GG_ABI_VERSION 11  /* 11: gg_adam_apply_dense, then gg_expected_g_grad, then gg_generator_dist_d and
-                              gg_expected_d_grad (additions: every older entry point keeps
+                              gg_expected_d_grad, then gg_best_response, gg_best_response_grad and gg_best_response_spmm
+                              (additions: every older entry point keeps
                               its signature and meaning, and _cabi.lib() refuses a library that lacks a declared symbol); 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
 
 /* walk status codes (per walk) */
@@ -259,6 +260,38 @@ int gg_expected_d_grad(int64_t n_node, int32_t ld, const float *emb, const float
                        const int32_t *raw_adj, int64_t n_roots, const int32_t *roots, const double *dist_d,
                        const double *p_void, const int32_t *root_ok, double *accept, double *grad_emb, double *grad_bias,
                        void *scratch, int64_t scratch_bytes, void *stream);
+
+/* The game value against the best discriminator (csrc/best_response.cu, DESIGN.md section 5.8): for the roots of g (the
+ * generator's G-mode law as gg_generator_dist computes it from g's fields, current father-removal bits), with
+ * p(a) = mult[e] / |graph[c]| for the walk-CSR entry e = (c -> a) and G(a) = fl(pi_c(a) pi_a(c)) (the bits of
+ * gg_generator_dist's dist[k, a]) at the depth-1 nodes a:
+ *   vstar[k] = -sum_a (p(a) log1p(G(a) / p(a)) + G(a) log1p(p(a) / G(a)))  (= max_D V_c(G, D) = 2 JSD(p || G) - log 4;
+ *              the G term is 0 where G(a) = 0),  hit[k] = sum_a G(a),
+ * both summed over c's walk-CSR entries in the order of DESIGN.md section 5.8.  ok[k] = 1 iff |graph[c]| > 0 and
+ * gg_generator_dist's root_ok is 1 (the bits of gg_game_value's ok); otherwise vstar[k] = hit[k] = 0.  raw_indptr: the raw
+ * CSR's [n_node + 1]; mult: device int32 [nnz], mult[e] = the count of adj[e] in the raw list of e's row.  Only the
+ * depth-1 lists are built.  scratch: device, at least gg_best_response_scratch_bytes(n_node, nnz, n_roots) bytes
+ * (host-only size computation; O(n_roots * (nnz + n_node))); n_roots * n_node < 2^31.  One cooperative launch. */
+int gg_best_response_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int64_t *bytes);
+int gg_best_response(const gg_walk_desc *g, const int64_t *raw_indptr, const int32_t *mult, double *vstar, double *hit,
+                     int32_t *ok, void *scratch, int64_t scratch_bytes, void *stream);
+/* gg_best_response, and the gradient of sum_{ok c} vstar_c with respect to g's rows and biases as per-entry coefficients
+ * ADDED to the caller's accumulators acc_coef and acc_bias (device fp64 [nnz]): the edge coefficient c_e on both entries of
+ * each tree edge, the bias coefficient on the receiving node's entry.  The roots are taken in the order given, each entry
+ * one fp64 chain: pass the roots in ascending id order (and chunks in order) for bits that do not depend on the order or
+ * the chunking.  rev: gg_reverse_entries' (a symmetric walk CSR).  gg_best_response_spmm turns the accumulators into the
+ * gradient.  scratch: gg_best_response_grad_scratch_bytes(n_node, nnz, n_roots) bytes (20 bytes per (root, node) more than
+ * gg_best_response's).  One cooperative launch with one grid barrier per ok root. */
+int gg_best_response_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int64_t *bytes);
+int gg_best_response_grad(const gg_walk_desc *g, const int64_t *raw_indptr, const int32_t *mult, const int32_t *rev,
+                          double *vstar, double *hit, int32_t *ok, double *acc_coef, double *acc_bias, void *scratch,
+                          int64_t scratch_bytes, void *stream);
+/* The gradient from gg_best_response_grad's accumulators, ADDED to grad_emb (device fp64 [n_node, ld]) and grad_bias
+ * (device fp64 [n_node]): row y, coordinate i, is one fp64 chain over y's walk-CSR entries e in entry order,
+ * acc = fma(-acc_coef[e], emb[adj[e]][i], acc), and the bias accb = accb - acc_bias[e] (zero coefficients skipped).  Pad
+ * columns stay exactly 0.  No scratch.  One launch. */
+int gg_best_response_spmm(int64_t n_node, int32_t ld, const int64_t *indptr, const int32_t *adj, const float *emb,
+                          const double *acc_coef, const double *acc_bias, double *grad_emb, double *grad_bias, void *stream);
 
 /* The exact expectation of the reference's generator step (csrc/value_gref.cu, DESIGN.md section 5.6): for the roots of g
  * (the generator's law as gg_generator_dist computes it from g's fields, G mode, current father-removal bits) and the
