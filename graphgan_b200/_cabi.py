@@ -59,6 +59,8 @@ SIGNATURES = {
     "gg_game_value_grad_d": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P, _P, _P, _I64, _P]),
     "gg_expected_g_grad_scratch_bytes": (C.c_int, [_I64, _I64, _I64, _I32, C.POINTER(_I64)]),
     "gg_expected_g_grad": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _I32, _P, _P, _P, _P, _P, _I64, _P]),
+    "gg_expected_g_moments_scratch_bytes": (C.c_int, [_I64, _I64, _I64, _I32, C.POINTER(_I64)]),
+    "gg_expected_g_moments": (C.c_int, [C.POINTER(WalkDesc), _P, _P, _I32, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P]),
     "gg_expected_d_grad_scratch_bytes": (C.c_int, [_I64, _I32, _I64, C.POINTER(_I64)]),
     "gg_expected_d_grad": (C.c_int, [_I64, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _P]),
     "gg_best_response_scratch_bytes": (C.c_int, [_I64, _I64, _I64, C.POINTER(_I64)]),

@@ -67,6 +67,9 @@ value_dcos = False                 # with value_roots > 0: the value line ends i
 value_jsd = False                  # with value_roots > 0: the value line ends in " jsd:<mean JSD> hit:<mean hit>" (after
                                     # dcos): G's exact Jensen-Shannon divergence from the data and its mass on the true
                                     # neighbours, from the top two levels of each tree (DESIGN.md section 5.8)
+value_gsnr = False                 # with value_roots > 0: the value line ends in " gsnr:<n |M|^2 / sum var_c>" (after jsd):
+                                    # the signal-to-noise ratio of one sampled G pass of n = n_sample_gen walks per root,
+                                    # exact (DESIGN.md section 5.9)
 exact_roots = 0                     # > 0: train() plays the exact game on this many seeded roots (DESIGN.md section 5.5):
                                     # each D / G step is an Adam step on the exact gradient of the mean V; no walks are
                                     # sampled.  Single process only.  0: the reference's sampled training

@@ -24,6 +24,18 @@
 // a in depth-first pre-order, children in entry order (a as the ancestor).  A list of at most 256 entries has chain_0 only.
 // Every term is one fma per coordinate with c = fl(rho * fl(kappa_up + kappa_dn)) (fp64), and one add of rho kappa for the
 // bias.
+//
+// The second moment of one walk's step (DESIGN.md section 5.9, gg_expected_g_moments) runs the same stages and then:
+// moment_kernel, an 8-lane group per item of depth >= 1, writes full(y) (the row depth(y) - w of y's path, complete
+// whatever the walk does below y) and tail(y) (the rows depth(y) - w + 1 .. depth(y), truncated at y) in fp64 from the
+// kappa planes and E_G rows of y's <= 2w ancestors; moment_prefix_kernel, top-down like reach_kernel, turns full into
+// Pf(y) = Pf(father(y)) + full(y) and tail into |s(y)|^2 = Pf(y) + tail(y); root_sum_kernel gives sq_c = sum_y P(y)
+// |s(y)|^2; gather_sq_kernel is gather_kernel that also stores each root's squared contribution to each row, and
+// root_sum_kernel reduces that plane to mn_c = |m_c|^2.
+//   row u (u levels above y): R = sum_v fl(kappa_up + kappa_dn) E_G[p_v] over the path nodes p_v within w of p_u, one
+//   fp64 fma chain per coordinate from +0 in path order (v descending); B = the same chain of the kappas into p_u; a lane's
+//   sum of R^2 over its coordinates gl, gl + 8, ... in order, then the group's xor butterfly 4, 2, 1; row = fl(R.R + B^2)
+//   tail(y) = rows u = min(w - 1, depth(y)) .. 0 in that order from +0
 #include <cooperative_groups.h>
 #include <math.h>
 
@@ -219,13 +231,15 @@ __device__ __forceinline__ void down_chain(const GrArgs &g, size_t o, const uint
 }
 
 // Work items: first one CTA per big node, then groups of 8 nodes, a warp per node (big nodes skipped).  Each item runs
-// the roots in order and stores its rows once.
-template <int CPL>
-__global__ void __launch_bounds__(GR_THREADS) gather_kernel(const GrArgs g) {
+// the roots in order and stores its rows once.  SQ: also mnp[k, a] = |root k's contribution to row a|^2 (coordinates,
+// then the bias squared), with a fixed block reduction on the big-node path; the caller clears mnp.
+template <int CPL, bool SQ>
+__device__ __forceinline__ void gather_rows(const GrArgs &g, double *mnp) {
     constexpr int LD = 32 * CPL;
     extern __shared__ __align__(16) unsigned char gr_smem[];
     double *s_ch = reinterpret_cast<double *>(gr_smem);   // [GR_CHAINS, LD] chain sums, then [GR_CHAINS] bias chains
     double *s_chb = s_ch + GR_CHAINS * LD;
+    double *s_sq = s_chb + GR_CHAINS;                      // SQ: [GR_CHAINS] warp partials of the squared contribution
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const long long n_big = *g.big_cnt, n_groups = (g.n_node + GR_CHAINS - 1) / GR_CHAINS;
     for (long long item = blockIdx.x; item < n_big + n_groups; item += gridDim.x) {
@@ -264,20 +278,33 @@ __global__ void __launch_bounds__(GR_THREADS) gather_kernel(const GrArgs g) {
                     }
                     x = g.father[o + x];
                 }
+                double qs = 0.0, cb = 0.0;
 #pragma unroll
                 for (int r = 0; r < 2; ++r) {
                     const int j = threadIdx.x + GR_THREADS * r;
                     if (j >= LD) continue;
                     double ch = s_ch[j];
                     for (int q = 1; q < GR_CHAINS; ++q) ch = __dadd_rn(ch, s_ch[q * LD + j]);
-                    acc[r] = __dadd_rn(acc[r], __dadd_rn(up[r], ch));
+                    const double cr = __dadd_rn(up[r], ch);
+                    acc[r] = __dadd_rn(acc[r], cr);
+                    if (SQ) qs = __fma_rn(cr, cr, qs);
+                }
+                if (SQ) {
+                    qs = warp_dsum(qs);
+                    if (lane == 0) s_sq[wid] = qs;
                 }
                 if (threadIdx.x == 0) {
                     double chb = s_chb[0];
                     for (int q = 1; q < GR_CHAINS; ++q) chb = __dadd_rn(chb, s_chb[q]);
-                    accb = __dadd_rn(accb, __dadd_rn(upb, chb));
+                    cb = __dadd_rn(upb, chb);
+                    accb = __dadd_rn(accb, cb);
                 }
                 __syncthreads();
+                if (SQ && threadIdx.x == 0) {       // s_sq is next written after the next root's first barrier
+                    double t = s_sq[0];
+                    for (int w = 1; w < GR_CHAINS; ++w) t = __dadd_rn(t, s_sq[w]);
+                    mnp[o + a] = __dadd_rn(t, __dmul_rn(cb, cb));
+                }
             }
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
@@ -315,9 +342,19 @@ __global__ void __launch_bounds__(GR_THREADS) gather_kernel(const GrArgs g) {
                 for (int i = 0; i < CPL; ++i) up[i] = __fma_rn(c, (double)__ldg(g.emb + (size_t)x * LD + lane + 32 * i), up[i]);
                 x = g.father[o + x];
             }
+            double qs = 0.0;
 #pragma unroll
-            for (int i = 0; i < CPL; ++i) acc[i] = __dadd_rn(acc[i], __dadd_rn(up[i], s[i]));
-            accb = __dadd_rn(accb, __dadd_rn(upb, sb));
+            for (int i = 0; i < CPL; ++i) {
+                const double ci = __dadd_rn(up[i], s[i]);
+                acc[i] = __dadd_rn(acc[i], ci);
+                if (SQ) qs = __fma_rn(ci, ci, qs);
+            }
+            const double cb = __dadd_rn(upb, sb);
+            accb = __dadd_rn(accb, cb);
+            if (SQ) {
+                qs = warp_dsum(qs);
+                if (lane == 0) mnp[o + a] = __dadd_rn(qs, __dmul_rn(cb, cb));
+            }
         }
 #pragma unroll
         for (int i = 0; i < CPL; ++i) g.grad_emb[(size_t)a * LD + lane + 32 * i] = acc[i];
@@ -326,17 +363,154 @@ __global__ void __launch_bounds__(GR_THREADS) gather_kernel(const GrArgs g) {
 }
 
 template <int CPL>
-int launch_gather(const GrArgs &g, cudaStream_t st) {
-    const size_t smem = (size_t)GR_CHAINS * (32 * CPL + 1) * sizeof(double);
-    GG_CHECK(cudaFuncSetAttribute(gather_kernel<CPL>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+__global__ void __launch_bounds__(GR_THREADS) gather_kernel(const GrArgs g) { gather_rows<CPL, false>(g, nullptr); }
+
+template <int CPL>
+__global__ void __launch_bounds__(GR_THREADS) gather_sq_kernel(const GrArgs g, double *mnp) { gather_rows<CPL, true>(g, mnp); }
+
+// gather_kernel, or gather_sq_kernel when mnp is given
+template <int CPL>
+int launch_gather(const GrArgs &g, double *mnp, cudaStream_t st) {
+    const size_t smem = (size_t)GR_CHAINS * (32 * CPL + (mnp ? 2 : 1)) * sizeof(double);
+    const void *fn = mnp ? (const void *)gather_sq_kernel<CPL> : (const void *)gather_kernel<CPL>;
+    GG_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gather_kernel<CPL>, GR_THREADS, smem));
+    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, GR_THREADS, smem));
     GG_REQUIRE(per_sm >= 1, "expected G step gather kernel does not fit on an SM");
     const long long n_groups = (g.n_node + GR_CHAINS - 1) / GR_CHAINS;
     long long grid = (long long)sm_count() * per_sm;
     if (grid > n_groups + g.n_node) grid = n_groups + g.n_node;
-    gather_kernel<CPL><<<(unsigned)grid, GR_THREADS, smem, st>>>(g);
+    if (mnp)
+        gather_sq_kernel<CPL><<<(unsigned)grid, GR_THREADS, smem, st>>>(g, mnp);
+    else
+        gather_kernel<CPL><<<(unsigned)grid, GR_THREADS, smem, st>>>(g);
     return check_cuda(cudaGetLastError(), "expected G step gather launch");
+}
+
+int gather(const GrArgs &g, double *mnp, cudaStream_t st) {
+    switch (g.ld / 32) {
+        case 1: return launch_gather<1>(g, mnp, st);
+        case 2: return launch_gather<2>(g, mnp, st);
+        case 4: return launch_gather<4>(g, mnp, st);
+        case 8: return launch_gather<8>(g, mnp, st);
+        default: return launch_gather<16>(g, mnp, st);
+    }
+}
+
+// ---- section 5.9: the second moment of one walk's step
+struct GmArgs {
+    GrArgs g;
+    const double *dist;                        // the stop law P(y)
+    double *pf;                                // [n_roots, n_node]: full(y), then Pf(y); later gather_sq_kernel's plane
+    double *sqn;                               // [n_roots, n_node]: tail(y), then |s(y)|^2 (0 at the root and unreached)
+};
+
+constexpr int GM_PATH = 2 * GR_WMAX + 1;       // y and its ancestors up to 2w levels above it
+
+// fl(R.R + B^2) of row u of y's path (p[v]: the node v levels above y, v <= lc = min(depth(y), 2w)); see the top of the
+// file.  The pair (p_v, p_u) has its kappa planes at its deeper node, distance |u - v|.
+__device__ __forceinline__ double path_row(const GrArgs &g, size_t o, const int (&p)[GM_PATH], int u, int lc, int gl,
+                                           unsigned gmask) {
+    const int lo = u > g.window ? u - g.window : 0, hi = u + g.window < lc ? u + g.window : lc;
+    int pu = p[0];
+#pragma unroll
+    for (int v = 1; v < GM_PATH; ++v)
+        if (v == u) pu = p[v];
+    double cf[GM_PATH], b = 0.0;
+    unsigned live = 0u;
+#pragma unroll
+    for (int v = GM_PATH - 1; v >= 0; --v) {
+        cf[v] = 0.0;
+        if (v < lo || v > hi || v == u) continue;
+        live |= 1u << v;
+        const int deep = v < u ? p[v] : pu;
+        const size_t at = (size_t)((v < u ? u - v : v - u) - 1) * (size_t)g.rn + o + deep;
+        const float ku = g.kup[at], kd = g.kdn[at];
+        cf[v] = __dadd_rn((double)ku, (double)kd);
+        b = __dadd_rn(b, (double)(v < u ? kd : ku));      // kappa(p_v, p_u)
+    }
+    double q = 0.0;
+    for (int c = gl; c < g.ld; c += 8) {
+        double r = 0.0;
+#pragma unroll
+        for (int v = GM_PATH - 1; v >= 0; --v)
+            if (live >> v & 1u) r = __fma_rn(cf[v], (double)__ldg(g.emb + (size_t)p[v] * g.ld + c), r);
+        q = __fma_rn(r, r, q);
+    }
+#pragma unroll
+    for (int off = 4; off >= 1; off >>= 1) q = __dadd_rn(q, __shfl_xor_sync(gmask, q, off));
+    return __dadd_rn(q, __dmul_rn(b, b));
+}
+
+// an 8-lane group per item of depth >= 1: pf = full(y), sqn = tail(y)
+__global__ void __launch_bounds__(GR_THREADS) moment_kernel(const GmArgs m) {
+    const GrArgs &g = m.g;
+    const int lane = threadIdx.x & 31, gl = lane & 7;
+    const unsigned gmask = 0xffu << (lane & 24);
+    const long long gid = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 3, ng = ((long long)gridDim.x * blockDim.x) >> 3;
+    const long long i0 = g.lev_off[1 < *g.n_lev ? 1 : *g.n_lev], i1 = g.lev_off[*g.n_lev];
+    for (long long i = i0 + gid; i < i1; i += ng) {
+        const int4 it = g.items[i];
+        if (__ldg(g.ok + it.x) != 1) continue;
+        const size_t o = (size_t)it.x * (size_t)g.n_node;
+        int p[GM_PATH], lc = 0;
+        p[0] = it.y;
+#pragma unroll
+        for (int v = 1; v < GM_PATH; ++v) {
+            p[v] = (v <= 2 * g.window && p[v - 1] >= 0) ? (v == 1 ? it.z : g.father[o + p[v - 1]]) : -1;
+            if (p[v] >= 0) lc = v;
+        }
+        const double full = lc >= g.window ? path_row(g, o, p, g.window, lc, gl, gmask) : 0.0;
+        double tail = 0.0;
+        for (int u = g.window - 1 < lc ? g.window - 1 : lc; u >= 0; --u) tail = __dadd_rn(tail, path_row(g, o, p, u, lc, gl, gmask));
+        if (gl == 0) {
+            m.pf[o + it.y] = full;
+            m.sqn[o + it.y] = tail;
+        }
+    }
+}
+
+// top-down over the recorded levels (reach_kernel's shape): Pf(y) = Pf(father) + full(y), |s(y)|^2 = Pf(y) + tail(y)
+__global__ void __launch_bounds__(GR_THREADS) moment_prefix_kernel(const GmArgs m) {
+    cg::grid_group grid = cg::this_grid();
+    const GrArgs &g = m.g;
+    const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
+    const int n_lev = (int)*g.n_lev;
+    for (int lev = 1; lev < n_lev; ++lev) {
+        const long long i0 = g.lev_off[lev], i1 = g.lev_off[lev + 1];
+        for (long long i = i0 + tid; i < i1; i += nt) {
+            const int4 it = g.items[i];
+            if (__ldg(g.ok + it.x) != 1) continue;
+            const size_t o = (size_t)it.x * (size_t)g.n_node;
+            const double pf = __dadd_rn(m.pf[o + it.z], m.pf[o + it.y]);
+            m.pf[o + it.y] = pf;
+            m.sqn[o + it.y] = __dadd_rn(pf, m.sqn[o + it.y]);
+        }
+        grid.sync();
+    }
+}
+
+// out[k] = sum_v fl(w[k, v] x[k, v]) (w null: sum_v x[k, v]) over an ok root's nodes in npairs_kernel's order; 0 else
+__global__ void __launch_bounds__(GR_THREADS) root_sum_kernel(const GrArgs g, const double *w, const double *x, double *out) {
+    __shared__ double s_w[GR_CHAINS];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    for (long long k = blockIdx.x; k < g.n_roots; k += gridDim.x) {
+        double s = 0.0;
+        if (__ldg(g.ok + k) == 1) {
+            const size_t o = (size_t)k * (size_t)g.n_node;
+            for (long long v = threadIdx.x; v < g.n_node; v += GR_THREADS)
+                s = __dadd_rn(s, w ? __dmul_rn(w[o + v], x[o + v]) : x[o + v]);
+        }
+        s = warp_dsum(s);
+        if (lane == 0) s_w[wid] = s;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double t = s_w[0];
+            for (int q = 1; q < GR_CHAINS; ++q) t = __dadd_rn(t, s_w[q]);
+            out[k] = t;
+        }
+        __syncthreads();
+    }
 }
 
 struct GrLayout {
@@ -345,9 +519,10 @@ struct GrLayout {
     float *kup, *kdn;
     int *father, *root_ok, *big;
     unsigned *big_cnt;
+    double *pf, *sqn;                          // moments only
 };
 
-size_t gr_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, int window, GrLayout *v) {
+size_t gr_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, int window, bool moments, GrLayout *v) {
     size_t off = 0;
     auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
     const size_t rn = (size_t)n_roots * (size_t)n_node;
@@ -357,6 +532,7 @@ size_t gr_layout(void *buf, long long n_node, long long nnz_words, long long n_r
     const size_t o_kup = take((size_t)window * rn * sizeof(float)), o_kdn = take((size_t)window * rn * sizeof(float));
     const size_t o_fa = take(rn * sizeof(int)), o_ok = take((size_t)n_roots * sizeof(int));
     const size_t o_big = take((size_t)n_node * sizeof(int)), o_bc = take(sizeof(unsigned));
+    const size_t o_pf = moments ? take(rn * sizeof(double)) : 0, o_sqn = moments ? take(rn * sizeof(double)) : 0;
     if (buf && v) {
         unsigned char *b = static_cast<unsigned char *>(buf);
         v->rec = b + o_rec;
@@ -370,51 +546,49 @@ size_t gr_layout(void *buf, long long n_node, long long nnz_words, long long n_r
         v->root_ok = reinterpret_cast<int *>(b + o_ok);
         v->big = reinterpret_cast<int *>(b + o_big);
         v->big_cnt = reinterpret_cast<unsigned *>(b + o_bc);
+        v->pf = moments ? reinterpret_cast<double *>(b + o_pf) : nullptr;
+        v->sqn = moments ? reinterpret_cast<double *>(b + o_sqn) : nullptr;
     }
     return off;
 }
 
-}  // namespace
-}  // namespace gg
+struct GmOut {
+    double *sq, *mn, *sq_node;
+};
 
-extern "C" int gg_expected_g_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int32_t window,
-                                                int64_t *bytes) {
-    GG_REQUIRE(bytes && n_node >= 0 && nnz >= 0 && n_roots >= 0, "bad arguments");
-    GG_REQUIRE(window >= 1 && window <= gg::GR_WMAX, "window must be 1 .. 8");
-    *bytes = (int64_t)gg::gr_layout(nullptr, n_node, (nnz + 31) / 32, n_roots, window, nullptr);
-    return 0;
-}
-
-extern "C" int gg_expected_g_grad(const gg_walk_desc *gp, const float *d_emb, const float *d_bias, int32_t window,
-                                  double *n_pairs, int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch,
-                                  int64_t scratch_bytes, void *stream) {
+// gg_expected_g_grad's launch sequence; with mo, also gg_expected_g_moments' stages
+int expected_g_run(const gg_walk_desc *gp, const float *d_emb, const float *d_bias, int32_t window, double *n_pairs,
+                   int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes, void *stream,
+                   const GmOut *mo) {
     GG_REQUIRE(gp, "null descriptor");
     const gg_walk_desc &d = *gp;
-    GG_REQUIRE(gg::ld_supported(d.ld), GG_LD_MESSAGE);
-    GG_REQUIRE(window >= 1 && window <= gg::GR_WMAX, "window must be 1 .. 8");
+    GG_REQUIRE(ld_supported(d.ld), GG_LD_MESSAGE);
+    GG_REQUIRE(window >= 1 && window <= GR_WMAX, "window must be 1 .. 8");
     GG_REQUIRE(d.n_roots >= 0, "n_roots must be >= 0");
     if (d.n_roots == 0) return 0;
     GG_REQUIRE(d.n_node > 0 && d.emb && d.bias && d.indptr && d.adj && d.roots && d.tree_bits, "null graph/embedding pointer");
     GG_REQUIRE(d.tree_words > 0, "tree_words missing (gg_tree_words)");
     GG_REQUIRE(d_emb && d_bias, "null discriminator pointer");
     GG_REQUIRE(n_pairs && root_ok && grad_emb && grad_bias && scratch, "null output or scratch pointer");
+    GG_REQUIRE(!mo || (mo->sq && mo->mn), "null sq / mn pointer");
     GG_REQUIRE(d.n_roots * d.n_node < (1ll << 31), "n_roots * n_node must be below 2^31 (process the roots in chunks)");
-    GG_REQUIRE(!d.edge_score || (d.hub_threshold > 0 && d.hub_threshold < gg::SMEM_CAP), "hub_threshold out of range");
-    gg::GrLayout v;
-    const size_t need = gg::gr_layout(scratch, d.n_node, d.tree_words - 1, d.n_roots, window, &v);
-    GG_REQUIRE(scratch_bytes >= (int64_t)need, "scratch too small (gg_expected_g_grad_scratch_bytes)");
+    GG_REQUIRE(!d.edge_score || (d.hub_threshold > 0 && d.hub_threshold < SMEM_CAP), "hub_threshold out of range");
+    GrLayout v;
+    const size_t need = gr_layout(scratch, d.n_node, d.tree_words - 1, d.n_roots, window, mo != nullptr, &v);
+    GG_REQUIRE(scratch_bytes >= (int64_t)need, mo ? "scratch too small (gg_expected_g_moments_scratch_bytes)"
+                                                  : "scratch too small (gg_expected_g_grad_scratch_bytes)");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t rn = (size_t)d.n_roots * (size_t)d.n_node;
     GG_CHECK(cudaMemsetAsync(v.dist, 0, rn * sizeof(double), st));
     GG_CHECK(cudaMemsetAsync(root_ok, 0, (size_t)d.n_roots * sizeof(int32_t), st));
     GG_CHECK(cudaMemsetAsync(v.father, 0xff, rn * sizeof(int), st));
     GG_CHECK(cudaMemsetAsync(v.big_cnt, 0, sizeof(unsigned), st));
-    gg::GdRec rec;
+    GdRec rec;
     rec.pi_in = v.pi_in; rec.pi_stop = v.pi_stop; rec.father = v.father;
-    gg::gdist_rec_layout(v.rec, d.n_node, d.tree_words - 1, d.n_roots, &rec);
-    int rc = gg::gdist_rec_launch(d, v.dist, root_ok, rec, v.rec, st);
+    gdist_rec_layout(v.rec, d.n_node, d.tree_words - 1, d.n_roots, &rec);
+    int rc = gdist_rec_launch(d, v.dist, root_ok, rec, v.rec, st);
     if (rc) return rc;
-    gg::GrArgs g;
+    GrArgs g;
     g.n_node = d.n_node; g.n_roots = d.n_roots; g.tree_words = d.tree_words; g.rn = (long long)rn;
     g.ld = d.ld; g.window = window;
     g.indptr = (const long long *)d.indptr; g.adj = d.adj; g.roots = d.roots; g.ok = root_ok; g.tree_bits = d.tree_bits;
@@ -425,23 +599,73 @@ extern "C" int gg_expected_g_grad(const gg_walk_desc *gp, const float *d_emb, co
     g.n_pairs = n_pairs; g.grad_emb = grad_emb; g.grad_bias = grad_bias;
     {
         int per_sm = 0;
-        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gg::reach_kernel, gg::GR_THREADS, 0));
+        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, reach_kernel, GR_THREADS, 0));
         GG_REQUIRE(per_sm >= 1, "expected G step reach kernel does not fit on an SM");
         void *args[] = {(void *)&g};
-        GG_CHECK(cudaLaunchCooperativeKernel((const void *)gg::reach_kernel, dim3((unsigned)(gg::sm_count() * per_sm)),
-                                             dim3(gg::GR_THREADS), args, 0, st));
+        GG_CHECK(cudaLaunchCooperativeKernel((const void *)reach_kernel, dim3((unsigned)(sm_count() * per_sm)),
+                                             dim3(GR_THREADS), args, 0, st));
     }
-    gg::score_kernel<<<(unsigned)(gg::sm_count() * 8), gg::GR_THREADS, 0, st>>>(g);
+    score_kernel<<<(unsigned)(sm_count() * 8), GR_THREADS, 0, st>>>(g);
     GG_CHECK(cudaGetLastError());
-    gg::npairs_kernel<<<(unsigned)(d.n_roots < gg::sm_count() * 4 ? d.n_roots : gg::sm_count() * 4), gg::GR_THREADS, 0, st>>>(g);
+    const unsigned root_grid = (unsigned)(d.n_roots < sm_count() * 4 ? d.n_roots : sm_count() * 4);
+    npairs_kernel<<<root_grid, GR_THREADS, 0, st>>>(g);
     GG_CHECK(cudaGetLastError());
-    gg::big_nodes_kernel<<<(unsigned)((d.n_node + 255) / 256), 256, 0, st>>>(g);
+    big_nodes_kernel<<<(unsigned)((d.n_node + 255) / 256), 256, 0, st>>>(g);
     GG_CHECK(cudaGetLastError());
-    switch (d.ld / 32) {
-        case 1: return gg::launch_gather<1>(g, st);
-        case 2: return gg::launch_gather<2>(g, st);
-        case 4: return gg::launch_gather<4>(g, st);
-        case 8: return gg::launch_gather<8>(g, st);
-        default: return gg::launch_gather<16>(g, st);
+    if (!mo) return gather(g, nullptr, st);
+    GmArgs m;
+    m.g = g; m.dist = v.dist; m.pf = v.pf; m.sqn = mo->sq_node ? mo->sq_node : v.sqn;
+    GG_CHECK(cudaMemsetAsync(m.pf, 0, rn * sizeof(double), st));
+    GG_CHECK(cudaMemsetAsync(m.sqn, 0, rn * sizeof(double), st));
+    moment_kernel<<<(unsigned)(sm_count() * 8), GR_THREADS, 0, st>>>(m);
+    GG_CHECK(cudaGetLastError());
+    {
+        int per_sm = 0;
+        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, moment_prefix_kernel, GR_THREADS, 0));
+        GG_REQUIRE(per_sm >= 1, "expected G moments prefix kernel does not fit on an SM");
+        void *args[] = {(void *)&m};
+        GG_CHECK(cudaLaunchCooperativeKernel((const void *)moment_prefix_kernel, dim3((unsigned)(sm_count() * per_sm)),
+                                             dim3(GR_THREADS), args, 0, st));
     }
+    root_sum_kernel<<<root_grid, GR_THREADS, 0, st>>>(g, m.dist, m.sqn, mo->sq);
+    GG_CHECK(cudaGetLastError());
+    GG_CHECK(cudaMemsetAsync(m.pf, 0, rn * sizeof(double), st));             // Pf is spent: the plane of mn's terms
+    rc = gather(g, m.pf, st);
+    if (rc) return rc;
+    root_sum_kernel<<<root_grid, GR_THREADS, 0, st>>>(g, nullptr, m.pf, mo->mn);
+    return check_cuda(cudaGetLastError(), "expected G moments mn launch");
+}
+
+}  // namespace
+}  // namespace gg
+
+extern "C" int gg_expected_g_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int32_t window,
+                                                int64_t *bytes) {
+    GG_REQUIRE(bytes && n_node >= 0 && nnz >= 0 && n_roots >= 0, "bad arguments");
+    GG_REQUIRE(window >= 1 && window <= gg::GR_WMAX, "window must be 1 .. 8");
+    *bytes = (int64_t)gg::gr_layout(nullptr, n_node, (nnz + 31) / 32, n_roots, window, false, nullptr);
+    return 0;
+}
+
+extern "C" int gg_expected_g_grad(const gg_walk_desc *gp, const float *d_emb, const float *d_bias, int32_t window,
+                                  double *n_pairs, int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch,
+                                  int64_t scratch_bytes, void *stream) {
+    return gg::expected_g_run(gp, d_emb, d_bias, window, n_pairs, root_ok, grad_emb, grad_bias, scratch, scratch_bytes,
+                              stream, nullptr);
+}
+
+extern "C" int gg_expected_g_moments_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int32_t window,
+                                                   int64_t *bytes) {
+    GG_REQUIRE(bytes && n_node >= 0 && nnz >= 0 && n_roots >= 0, "bad arguments");
+    GG_REQUIRE(window >= 1 && window <= gg::GR_WMAX, "window must be 1 .. 8");
+    *bytes = (int64_t)gg::gr_layout(nullptr, n_node, (nnz + 31) / 32, n_roots, window, true, nullptr);
+    return 0;
+}
+
+extern "C" int gg_expected_g_moments(const gg_walk_desc *gp, const float *d_emb, const float *d_bias, int32_t window,
+                                     double *n_pairs, int32_t *root_ok, double *sq, double *mn, double *sq_node,
+                                     double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes, void *stream) {
+    const gg::GmOut mo{sq, mn, sq_node};
+    return gg::expected_g_run(gp, d_emb, d_bias, window, n_pairs, root_ok, grad_emb, grad_bias, scratch, scratch_bytes,
+                              stream, &mo);
 }

@@ -171,6 +171,15 @@ class GraphGAN(object):
         return self.sampler.expected_g_grad(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots),
                                             window=config.window_size)
 
+    def expected_g_moments(self, roots):
+        """expected_g_grad(roots) and the second moment of one walk's step per root (DESIGN.md section 5.9), with
+        config.window_size and the current models: sampler.WalkSampler.expected_g_moments.  Returns device (n_pairs,
+        root_ok, sq fp64, mn fp64, grad_emb fp64 [N, ld], grad_bias fp64 [N])."""
+        roots = np.asarray(roots.cpu() if isinstance(roots, self.torch.Tensor) else roots, np.int32).reshape(-1)
+        g, d = self.generator, self.discriminator
+        return self.sampler.expected_g_moments(g.emb, g.bias_t, d.emb, d.bias_t, self._trees_of(roots),
+                                               window=config.window_size)
+
     def expected_d_grad(self, roots):
         """The exact expectation of the reference's discriminator step of one pass over ``roots`` (DESIGN.md section 5.7),
         with the current models: sampler.WalkSampler.expected_d_grad.  Returns device (accept fp64, p_void fp64, ok_ref
@@ -235,7 +244,10 @@ class GraphGAN(object):
         gradient of the sum of V (game_value_grad_d; computed for it alone when value_grad_d is off).  A positive value
         means the reference's D step ascends V on average.  With config.value_jsd, " jsd:<mean JSD> hit:<mean hit>" comes
         last: the Jensen-Shannon divergence of the generator from the data and the generator's mass on the true
-        neighbours (best_response), means over the roots whose best-response ok is 1."""
+        neighbours (best_response), means over the roots whose best-response ok is 1.  With config.value_gsnr,
+        " gsnr:<snr>" comes last: n |M|^2 / sum_c var_c over the ok roots (expected_g_moments), n = config.n_sample_gen,
+        M = sum_c m_c the expected step of the reference's G pass and var_c = sq_c - mn_c the trace of the covariance of
+        one walk's step: the signal-to-noise ratio of one sampled G pass (nan without ok roots or when sum var_c <= 0)."""
         vg, vd = getattr(config, "value_grad", False), getattr(config, "value_grad_d", False)
         if vg:
             pos, neg, ok, g_emb, g_bias = self.game_value_grad(self.value_roots())
@@ -281,6 +293,13 @@ class GraphGAN(object):
             nb = int(sb.sum())
             jsd = float((vs[sb] / 2 + np.log(2.0)).mean()) if nb else np.nan
             line += " jsd:%r hit:%r" % (jsd, float(ht[sb].mean()) if nb else np.nan)
+        if getattr(config, "value_gsnr", False):
+            _, okg, sq, mn, r_emb, r_bias = self.expected_g_moments(self.value_roots())
+            sg = (okg == 1).cpu().numpy()
+            var = float((sq - mn).cpu().numpy()[sg].sum())
+            k = self.generator.n_emb
+            m2 = float((r_emb[:, :k] ** 2).sum().item() + (r_bias ** 2).sum().item())
+            line += " gsnr:%r" % (int(config.n_sample_gen) * m2 / var if sg.any() and var > 0 else np.nan)
         return line + "\n"
 
     # ------------------------------------------------------------------ training on the exact game (DESIGN.md section 5.5)

@@ -177,6 +177,14 @@ class WalkPlan:
         return self._s1
 
 
+def _gref_window(window):
+    """the window of expected_g_grad / expected_g_moments: config.window_size's range, 1 .. 8"""
+    window = int(window)
+    if not 1 <= window <= 8:
+        raise ValueError("window must be 1 .. 8, got %d" % window)
+    return window
+
+
 class WalkSampler:
     def __init__(self, graph, hub_threshold=128, depth1=True, hub_first=True, tma=True):
         import torch
@@ -575,9 +583,29 @@ class WalkSampler:
         The roots are taken in ascending id order (stable for duplicates), in chunks under the budget rule of
         ``distribution`` (``max_scratch_bytes``, default 2 GiB or env GG_GDIST_SCRATCH), each coordinate one fp64 chain
         over the roots: the bits do not depend on the chunking, the order of the roots or the call."""
-        window = int(window)
-        if not 1 <= window <= 8:
-            raise ValueError("window must be 1 .. 8, got %d" % window)
+        window = _gref_window(window)
+        n_pairs, ok, _, _, grad_emb, grad_bias, _ = self._expected_g(g_emb, g_bias, d_emb, d_bias, trees, window,
+                                                                     max_scratch_bytes, reuse, False, False)
+        return n_pairs, ok, grad_emb, grad_bias
+
+    def expected_g_moments(self, g_emb, g_bias, d_emb, d_bias, trees, *, window, max_scratch_bytes=None, reuse=None,
+                           per_node=False):
+        """``expected_g_grad`` and the second moment of one G walk's step (DESIGN.md section 5.9).  A walk that stops at y
+        adds the fixed vector s(y), the window-pair gradient of its body; per root c, sq_c = sum_y P(y) |s(y)|^2 and
+        mn_c = |m_c|^2, m_c the root's expected step (its share of grad_emb / grad_bias), norms over rows and biases.
+        sq_c - mn_c is the trace of the covariance of one walk's step, and a pass of n walks per root has
+        E|S|^2 = n^2 |sum_c m_c|^2 + n sum_c (sq_c - mn_c).
+        Returns device (n_pairs, root_ok, sq fp64 [R], mn fp64 [R], grad_emb, grad_bias), and with ``per_node`` also
+        sq_node fp64 [R, N] (|s(y)|^2 per node, 0 at the root and at nodes not reached), in the order of ``trees``.
+        n_pairs, root_ok, grad_emb and grad_bias are the bits of ``expected_g_grad``; the chunking and its budget are
+        the same (more scratch per root), and no bit depends on the chunking, the order of the roots or the call."""
+        window = _gref_window(window)
+        out = self._expected_g(g_emb, g_bias, d_emb, d_bias, trees, window, max_scratch_bytes, reuse, True, per_node)
+        return out if per_node else out[:6]
+
+    def _expected_g(self, g_emb, g_bias, d_emb, d_bias, trees, window, max_scratch_bytes, reuse, moments, per_node):
+        """the chunk loop of expected_g_grad (moments False) and expected_g_moments: (n_pairs, ok, sq, mn, grad_emb,
+        grad_bias, sq_node); sq / mn are None without moments, sq_node None without per_node"""
         torch, g = self.torch, self.g
         assert g_emb.dtype == torch.float32 and g_emb.is_contiguous() and g_bias.dtype == torch.float32
         assert d_emb.dtype == torch.float32 and d_emb.is_contiguous() and d_bias.dtype == torch.float32
@@ -585,32 +613,47 @@ class WalkSampler:
         R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
         n_pairs = torch.zeros(R, dtype=torch.float64, device=self.device)
         ok = torch.zeros(R, dtype=torch.int32, device=self.device)
+        sq, mn = (torch.zeros(R, dtype=torch.float64, device=self.device) for _ in range(2)) if moments else (None, None)
+        sq_node = torch.zeros((R, N), dtype=torch.float64, device=self.device) if per_node else None
         grad_emb = torch.zeros(tuple(g_emb.shape), dtype=torch.float64, device=self.device)
         grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
         if R == 0:
-            return n_pairs, ok, grad_emb, grad_bias
+            return n_pairs, ok, sq, mn, grad_emb, grad_bias, sq_node
         order = torch.argsort(trees.roots.long(), stable=True)
         st_trees = trees.select(order)
         reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
+        name = "gg_expected_g_moments" if moments else "gg_expected_g_grad"
+        size_fn = getattr(self.lib, name + "_scratch_bytes")
 
         def scratch_bytes(k):
             nb = C.c_int64(0)
-            _cabi.check(self.lib.gg_expected_g_grad_scratch_bytes(N, nnz, k, window, C.byref(nb)),
-                        "gg_expected_g_grad_scratch_bytes")
+            _cabi.check(size_fn(N, nnz, k, window, C.byref(nb)), name + "_scratch_bytes")
             return nb.value
         chunk = max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
         scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
         sn, so = torch.zeros_like(n_pairs), torch.zeros_like(ok)
+        ssq, smn = (torch.zeros_like(sq), torch.zeros_like(mn)) if moments else (None, None)
+        snode = torch.empty_like(sq_node) if per_node else None
         d = self._law_desc(g_emb, g_bias, st_trees, reuse, None)
         st = self._stream()
         for lo in range(0, R, chunk):
             hi = min(R, lo + chunk)
             d.n_roots, d.roots, d.tree_bits = hi - lo, ptr(st_trees.roots[lo:hi]), ptr(st_trees.tree_bits[lo:hi])
-            _cabi.check(self.lib.gg_expected_g_grad(C.byref(d), ptr(d_emb), ptr(d_bias), window, ptr(sn[lo:hi]), ptr(so[lo:hi]),
-                                                    ptr(grad_emb), ptr(grad_bias), ptr(scratch), scratch.numel(), st),
-                        "gg_expected_g_grad")
+            if moments:
+                rc = self.lib.gg_expected_g_moments(C.byref(d), ptr(d_emb), ptr(d_bias), window, ptr(sn[lo:hi]),
+                                                    ptr(so[lo:hi]), ptr(ssq[lo:hi]), ptr(smn[lo:hi]),
+                                                    ptr(snode[lo:hi]) if per_node else None, ptr(grad_emb), ptr(grad_bias),
+                                                    ptr(scratch), scratch.numel(), st)
+            else:
+                rc = self.lib.gg_expected_g_grad(C.byref(d), ptr(d_emb), ptr(d_bias), window, ptr(sn[lo:hi]), ptr(so[lo:hi]),
+                                                 ptr(grad_emb), ptr(grad_bias), ptr(scratch), scratch.numel(), st)
+            _cabi.check(rc, name)
         n_pairs[order], ok[order] = sn, so
-        return n_pairs, ok, grad_emb, grad_bias
+        if moments:
+            sq[order], mn[order] = ssq, smn
+        if per_node:
+            sq_node[order] = snode
+        return n_pairs, ok, sq, mn, grad_emb, grad_bias, sq_node
 
     # ------------------------------------------------------------------ expected reference D step
     def expected_d_grad(self, g_emb, g_bias, d_emb, d_bias, trees, *, max_scratch_bytes=None, reuse=None):

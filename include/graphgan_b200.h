@@ -29,7 +29,8 @@ extern "C" {
 #endif
 
 #define GG_ABI_VERSION 11  /* 11: gg_adam_apply_dense, then gg_expected_g_grad, then gg_generator_dist_d and
-                              gg_expected_d_grad, then gg_best_response, gg_best_response_grad and gg_best_response_spmm
+                              gg_expected_d_grad, then gg_best_response, gg_best_response_grad and gg_best_response_spmm,
+                              then gg_expected_g_moments
                               (additions: every older entry point keeps
                               its signature and meaning, and _cabi.lib() refuses a library that lacks a declared symbol); 10: gg_game_value_grad_d; 9: gg_game_value_grad; 8: gg_game_value; 7: gg_generator_dist */
 
@@ -313,6 +314,19 @@ int gg_expected_g_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_root
 int gg_expected_g_grad(const gg_walk_desc *g, const float *d_emb, const float *d_bias, int32_t window, double *n_pairs,
                        int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes,
                        void *stream);
+/* gg_expected_g_grad, and the second moment of one walk's step (csrc/value_gref.cu, DESIGN.md section 5.9).  A G walk
+ * that stops at y adds a fixed vector s(y), the window-pair gradient of the body root -> y; P(y) is gg_generator_dist's
+ * law.  Writes, per root, sq = sum_y P(y) |s(y)|^2 and mn = |m|^2 (device fp64 [n_roots]; 0 where root_ok = 0), m the
+ * root's expected step (its contribution to grad_emb / grad_bias); the norms run over the rows and the biases.  sq - mn
+ * is the trace of the covariance of one walk's step.  sq_node (device fp64 [n_roots, n_node], or NULL): |s(y)|^2 per
+ * node, 0 at the root and at nodes not reached.  n_pairs, root_ok, grad_emb and grad_bias are gg_expected_g_grad's, bit
+ * for bit, and the arguments are checked as there.  The bits depend on the inputs only.  scratch: device, at least
+ * gg_expected_g_moments_scratch_bytes(n_node, nnz, n_roots, window) bytes (host-only size computation;
+ * gg_expected_g_grad's plus 16 bytes per (root, node)). */
+int gg_expected_g_moments_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int32_t window, int64_t *bytes);
+int gg_expected_g_moments(const gg_walk_desc *g, const float *d_emb, const float *d_bias, int32_t window, double *n_pairs,
+                          int32_t *root_ok, double *sq, double *mn, double *sq_node, double *grad_emb, double *grad_bias,
+                          void *scratch, int64_t scratch_bytes, void *stream);
 
 /* prepare_data_for_d's output rows (graph_gan.py:192-201): for every accepted root, in batch
  * order: [i]*k + [i]*k | pos + neg | 1*k + 0*k.  row_ptr: device [R+1] scratch/out (exclusive
