@@ -19,14 +19,13 @@
 #include <cooperative_groups.h>
 #include <math.h>
 
-#include "walk_list.cuh"
+#include "exact.cuh"
 
 namespace gg {
 namespace {
 
 namespace cg = cooperative_groups;
 
-constexpr double BR_TWO53 = 9007199254740992.0;
 constexpr long long BR_BLOCK = 256;        // entries of a depth-1 node's row per unit of the coefficient pass
 
 struct BrView {
@@ -54,67 +53,25 @@ struct BrArgs {
 size_t br_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, bool grad, BrView *v) {
     const long long stride = 32 * nnz_words + n_node;   // >= nnz + n_node (nnz_words = gg_tree_words(nnz) - 1)
     const size_t rn = (size_t)n_roots * (size_t)n_node;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
-    const size_t o_cnt = take(sizeof(unsigned));
-    const size_t o_items = take(rn * sizeof(int4));
-    const size_t o_ids = take((size_t)n_roots * (size_t)stride * sizeof(int));
-    const size_t o_sc = take((size_t)n_roots * (size_t)stride * sizeof(float));
-    const size_t o_pica = take(rn * sizeof(double)), o_G = take(rn * sizeof(double));
-    const size_t o_hs = take(rn * sizeof(double)), o_pt = take(rn * sizeof(double));
-    const size_t o_ok = take((size_t)n_roots * sizeof(int)), o_H = take((size_t)n_roots * sizeof(double));
-    size_t o_wac = 0, o_pix = 0, o_boff = 0, o_nu = 0;
-    if (grad) {
-        o_wac = take(rn * sizeof(double));
-        o_pix = take(rn * sizeof(double));
-        o_boff = take(rn * sizeof(int));
-        o_nu = take((size_t)n_roots * sizeof(int));
-    }
-    if (buf && v) {
-        unsigned char *b = static_cast<unsigned char *>(buf);
-        v->cnt = reinterpret_cast<unsigned *>(b + o_cnt);
-        v->items = reinterpret_cast<int4 *>(b + o_items);
-        v->pool_ids = reinterpret_cast<int *>(b + o_ids);
-        v->pool_sc = reinterpret_cast<float *>(b + o_sc);
-        v->pool_stride = stride;
-        v->pi_ca = reinterpret_cast<double *>(b + o_pica);
-        v->G = reinterpret_cast<double *>(b + o_G);
-        v->hs = reinterpret_cast<double *>(b + o_hs);
-        v->pt = reinterpret_cast<double *>(b + o_pt);
-        v->root_ok = reinterpret_cast<int *>(b + o_ok);
-        v->H = reinterpret_cast<double *>(b + o_H);
-        v->wac = grad ? reinterpret_cast<double *>(b + o_wac) : nullptr;
-        v->pi_x = grad ? reinterpret_cast<double *>(b + o_pix) : nullptr;
-        v->boff = grad ? reinterpret_cast<int *>(b + o_boff) : nullptr;
-        v->nunit = grad ? reinterpret_cast<int *>(b + o_nu) : nullptr;
-    }
-    return off;
-}
-
-__device__ __forceinline__ bool br_bit(const uint32_t *tb, long long e) { return (__ldg(tb + (e >> 5)) >> (e & 31)) & 1u; }
-
-// lane l's value, then the xor butterfly 16, 8, 4, 2, 1 (every lane ends with the same bits)
-__device__ __forceinline__ double br_warp_dsum(double x) {
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) x = __dadd_rn(x, __shfl_xor_sync(FULL, x, off));
-    return x;
-}
-
-// pi of candidate j = t0 + lane of a list with n > 1 candidates (gdist_item's q -> pi, tile by tile; carry / k_prev
-// carry the tiles)
-__device__ __forceinline__ double br_pi_tile(const float *sc, int n, float S, double total, int t0, int lane, double &carry,
-                                             double &k_prev) {
-    const int j = t0 + lane;
-    double x = (j < n) ? (double)__fdiv_rn(sc[j], S) : 0.0;
-    x = warp_scan_ks(x, lane);
-    const double q = __ddiv_rn(__dadd_rn(carry, x), total);
-    const double k = ceil(__dmul_rn(q, BR_TWO53));
-    double kb = __shfl_up_sync(FULL, k, 1);
-    if (lane == 0) kb = k_prev;
-    const double pi = __dmul_rn(__dsub_rn(k, kb), 1.0 / BR_TWO53);
-    k_prev = __shfl_sync(FULL, k, 31);
-    carry = __dadd_rn(carry, __shfl_sync(FULL, x, 31));
-    return pi;
+    Slab s(buf);
+    BrView t;
+    t.cnt = s.take<unsigned>(1);
+    t.items = s.take<int4>(rn);
+    t.pool_ids = s.take<int>((size_t)n_roots * (size_t)stride);
+    t.pool_sc = s.take<float>((size_t)n_roots * (size_t)stride);
+    t.pool_stride = stride;
+    t.pi_ca = s.take<double>(rn);
+    t.G = s.take<double>(rn);
+    t.hs = s.take<double>(rn);
+    t.pt = s.take<double>(rn);
+    t.root_ok = s.take<int>((size_t)n_roots);
+    t.H = s.take<double>((size_t)n_roots);
+    t.wac = grad ? s.take<double>(rn) : nullptr;
+    t.pi_x = grad ? s.take<double>(rn) : nullptr;
+    t.boff = grad ? s.take<int>(rn) : nullptr;
+    t.nunit = grad ? s.take<int>((size_t)n_roots) : nullptr;
+    if (buf && v) *v = t;
+    return s.off;
 }
 
 // level 0: the root's list (its children), pi_c of every child; the reached children become depth-1 items
@@ -127,26 +84,16 @@ __device__ __forceinline__ void br_root_item(const gg_walk_desc &d, const BrView
     const long long a0 = d.indptr[c], a1 = d.indptr[c + 1];
     int *g_ids = v.pool_ids + (size_t)slot * (size_t)v.pool_stride + (size_t)(a0 + c);
     float *g_sc = v.pool_sc + (size_t)slot * (size_t)v.pool_stride + (size_t)(a0 + c);
-    int n;
-    float m;
-    int *ids;
-    float *sc;
-    build_list<CPL, UNR>(d, tb, c, -1, false, s_ids, s_sc, g_ids, g_sc, lane, n, m, ids, sc, rows, cyc, stg);
-    if (n == 0) return;                                      // no children: every walk voids, root_ok stays 0
+    ListLaw L = list_law<CPL>(d, tb, c, -1, false, s_ids, s_sc, g_ids, g_sc, lane, rows, cyc, stg);
+    if (L.n == 0) return;                                    // no children: every walk voids, root_ok stays 0
     if (lane == 0) v.root_ok[slot] = 1;
-    float S = 0.0f;
-    double total = 0.0;
-    if (n > 1) {
-        double car[2];
-        S = softmax_exp_sum<UNR_S1>(sc, n, m, lane);
-        total = cdf_total<UNR_S1>(sc, n, S, lane, car);
-    }
+    list_norm(L, lane);
     double carry = 0.0, k_prev = 0.0;
-    for (int t0 = 0; t0 < n; t0 += 32) {
-        const double pi = n > 1 ? br_pi_tile(sc, n, S, total, t0, lane, carry, k_prev) : 1.0;
+    for (int t0 = 0; t0 < L.n; t0 += 32) {
+        const double pi = L.n > 1 ? pi_tile(L, t0, lane, carry, k_prev) : 1.0;
         const int j = t0 + lane;
-        if (j < n) {
-            const size_t x = o + (size_t)ids[j];
+        if (j < L.n) {
+            const size_t x = o + (size_t)L.ids[j];
             v.pi_ca[x] = pi;                                 // reach(a) = fl(1 * pi_c(a)) = pi_c(a)
             v.G[x] = 0.0; v.hs[x] = 0.0; v.pt[x] = 0.0;     // (the item of a reached child overwrites them)
             if (v.wac) v.wac[x] = 0.0;
@@ -157,7 +104,7 @@ __device__ __forceinline__ void br_root_item(const gg_walk_desc &d, const BrView
         const long long e = e0 + lane;
         bool take = false;
         int child = -1, rm = 0;
-        if (e < a1 && br_bit(tb, e)) {
+        if (e < a1 && tree_bit(tb, e)) {
             child = __ldg(d.adj + e);
             take = v.pi_ca[o + child] > 0.0;
             rm = d.d1_bits ? (int)((__ldg(d.d1_bits + (e >> 5)) >> (e & 31)) & 1u) : 0;
@@ -180,31 +127,21 @@ __device__ __forceinline__ void br_d1_item(const gg_walk_desc &d, const BrArgs &
     const long long a0 = d.indptr[a], a1 = d.indptr[a + 1];
     if (it.w) {
         bool any = false;
-        for (long long e = a0 + lane; e < a1 && !any; e += 32) any = br_bit(tb, e);
+        for (long long e = a0 + lane; e < a1 && !any; e += 32) any = tree_bit(tb, e);
         if (!__any_sync(FULL, any) && lane == 0) v.root_ok[slot] = -1;
         return;
     }
     int *g_ids = v.pool_ids + (size_t)slot * (size_t)v.pool_stride + (size_t)(a0 + a);
     float *g_sc = v.pool_sc + (size_t)slot * (size_t)v.pool_stride + (size_t)(a0 + a);
-    int n;
-    float m;
-    int *ids;
-    float *sc;
-    build_list<CPL, UNR>(d, tb, a, c, true, s_ids, s_sc, g_ids, g_sc, lane, n, m, ids, sc, rows, cyc, stg);   // n >= 1
-    float S = 0.0f;
-    double total = 0.0;
-    if (n > 1) {
-        double car[2];
-        S = softmax_exp_sum<UNR_S1>(sc, n, m, lane);
-        total = cdf_total<UNR_S1>(sc, n, S, lane, car);
-    }
+    ListLaw L = list_law<CPL>(d, tb, a, c, true, s_ids, s_sc, g_ids, g_sc, lane, rows, cyc, stg);   // n >= 1
+    list_norm(L, lane);
     double carry = 0.0, k_prev = 0.0, pi_ac = 0.0;
-    for (int t0 = 0; t0 < n; t0 += 32) {
-        const double pi = n > 1 ? br_pi_tile(sc, n, S, total, t0, lane, carry, k_prev) : 1.0;
+    for (int t0 = 0; t0 < L.n; t0 += 32) {
+        const double pi = L.n > 1 ? pi_tile(L, t0, lane, carry, k_prev) : 1.0;
         const int j = t0 + lane;
         if (j == 0) pi_ac = pi;                              // the father's candidate: the stop step
         if constexpr (GRAD) {
-            if (j > 0 && j < n) v.pi_x[o + (size_t)ids[j]] = pi;
+            if (j > 0 && j < L.n) v.pi_x[o + (size_t)L.ids[j]] = pi;
         }
     }
     if (lane != 0) return;
@@ -221,7 +158,7 @@ __device__ __forceinline__ void br_d1_item(const gg_walk_desc &d, const BrArgs &
     if constexpr (GRAD) v.wac[o + a] = __dmul_rn(hs, __dsub_rn(1.0, pi_ac));
 }
 
-// the per-root sums over the root's row entries (lane l chains entries a0 + l, a0 + l + 32, ...; then br_warp_dsum);
+// the per-root sums over the root's row entries (lane l chains entries a0 + l, a0 + l + 32, ...; then warp_dsum);
 // with GRAD the unit offsets of the coefficient pass
 template <bool GRAD>
 __device__ __forceinline__ void br_root_sum(const gg_walk_desc &d, const BrArgs &ar, const BrView &v, int slot, int lane) {
@@ -233,7 +170,7 @@ __device__ __forceinline__ void br_root_sum(const gg_walk_desc &d, const BrArgs 
     double sg = 0.0, sh = 0.0, sv = 0.0;
     if (ok) {
         for (long long e = a0 + lane; e < a1; e += 32) {
-            if (!br_bit(tb, e)) continue;
+            if (!tree_bit(tb, e)) continue;
             const size_t x = o + (size_t)__ldg(d.adj + e);
             const double g = __ldcg(v.G + x), h = __ldcg(v.hs + x);
             sg = __dadd_rn(sg, g);
@@ -241,9 +178,9 @@ __device__ __forceinline__ void br_root_sum(const gg_walk_desc &d, const BrArgs 
             sv = __dadd_rn(sv, __dadd_rn(__ldcg(v.pt + x), h));
         }
     }
-    sg = br_warp_dsum(sg);
-    sh = br_warp_dsum(sh);
-    sv = br_warp_dsum(sv);
+    sg = warp_dsum(sg);
+    sh = warp_dsum(sh);
+    sv = warp_dsum(sv);
     if (lane == 0) {
         ar.ok[slot] = ok ? 1 : 0;
         ar.vstar[slot] = ok ? __dsub_rn(0.0, sv) : 0.0;
@@ -256,7 +193,7 @@ __device__ __forceinline__ void br_root_sum(const gg_walk_desc &d, const BrArgs 
         for (long long e0 = a0; e0 < a1; e0 += 32) {
             const long long e = e0 + lane;
             int nb = 0;
-            if (ok && e < a1 && br_bit(tb, e)) {
+            if (ok && e < a1 && tree_bit(tb, e)) {
                 const int x = __ldg(d.adj + e);
                 nb = 1;
                 if (__ldcg(v.hs + o + x) != 0.0) {
@@ -313,7 +250,7 @@ __device__ __forceinline__ void br_apply_unit(const gg_walk_desc &d, const BrArg
     const long long x0 = d.indptr[a] + BR_BLOCK * b, xe = d.indptr[a + 1];
     const long long x1 = x0 + BR_BLOCK < xe ? x0 + BR_BLOCK : xe;
     for (long long e2 = x0 + lane; e2 < x1; e2 += 32) {
-        if (!br_bit(tb, e2)) continue;
+        if (!tree_bit(tb, e2)) continue;
         const double p = __ldcg(v.pi_x + o + (size_t)__ldg(d.adj + e2));
         if (p == 0.0) continue;
         const double t = -__dmul_rn(p, h);                   // w_a(x); w_x(a) = 0 at depth 2
@@ -422,31 +359,6 @@ __global__ void __launch_bounds__(256) best_response_spmm_kernel(long long n_nod
     }
 }
 
-template <int CPL>
-int launch_spmm(long long n_node, const long long *indptr, const int *adj, const float *emb, const double *acc_coef,
-                const double *acc_bias, double *grad_emb, double *grad_bias, cudaStream_t st) {
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, best_response_spmm_kernel<CPL>, 256, 0));
-    GG_REQUIRE(per_sm >= 1, "best-response SpMM kernel does not fit on an SM");
-    long long grid = (long long)sm_count() * per_sm;
-    const long long need = (n_node + 7) / 8;
-    if (grid > need) grid = need;
-    best_response_spmm_kernel<CPL><<<(unsigned)grid, 256, 0, st>>>(n_node, indptr, adj, emb, acc_coef, acc_bias, grad_emb,
-                                                                   grad_bias);
-    return check_cuda(cudaGetLastError(), "best-response SpMM launch");
-}
-
-template <bool GRAD>
-const void *br_kernel_for(int ld) {
-    switch (ld / 32) {
-        case 1: return (const void *)best_response_kernel<1, GRAD>;
-        case 2: return (const void *)best_response_kernel<2, GRAD>;
-        case 4: return (const void *)best_response_kernel<4, GRAD>;
-        case 8: return (const void *)best_response_kernel<8, GRAD>;
-        default: return (const void *)best_response_kernel<16, GRAD>;
-    }
-}
-
 int br_run(const gg_walk_desc &d, const int64_t *raw_indptr, const int32_t *mult, const int32_t *rev, double *vstar,
            double *hit, int32_t *ok, double *acc_coef, double *acc_bias, void *scratch, int64_t scratch_bytes, bool grad,
            void *stream) {
@@ -460,34 +372,13 @@ int br_run(const gg_walk_desc &d, const int64_t *raw_indptr, const int32_t *mult
     BrArgs ar;
     ar.raw_indptr = (const long long *)raw_indptr; ar.mult = mult; ar.rev = rev;
     ar.vstar = vstar; ar.hit = hit; ar.ok = ok; ar.acc_coef = acc_coef; ar.acc_bias = acc_bias;
-    const void *kern = grad ? br_kernel_for<true>(d.ld) : br_kernel_for<false>(d.ld);
-    int dev = 0, coop = 0;
-    GG_CHECK(cudaGetDevice(&dev));
-    GG_CHECK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-    GG_REQUIRE(coop, "device does not support cooperative launches");
-    const int cpl = d.ld / 32, nt = WARPS_PER_CTA * 32;
-    const int smem = walk_smem_bytes(cpl, WARPS_PER_CTA);
-    GG_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, nt, smem));
-    GG_REQUIRE(per_sm >= 1, "best-response kernel does not fit on an SM");
-    if (per_sm > walk_min_ctas(cpl)) per_sm = walk_min_ctas(cpl);
+    const void *kern = with_cpl(d.ld, [grad](auto c) {
+        return grad ? (const void *)best_response_kernel<c, true> : (const void *)best_response_kernel<c, false>;
+    });
+    const int cpl = d.ld / 32;
     void *args[] = {(void *)&d, (void *)&ar, (void *)&v};
-    GG_CHECK(cudaLaunchCooperativeKernel(kern, dim3((unsigned)(sm_count() * per_sm)), dim3(nt), args, (size_t)smem, st));
-    return 0;
-}
-
-int br_check_desc(const gg_walk_desc *dp) {
-    GG_REQUIRE(dp, "null descriptor");
-    const gg_walk_desc &d = *dp;
-    GG_REQUIRE(ld_supported(d.ld), GG_LD_MESSAGE);
-    GG_REQUIRE(d.n_roots >= 0, "n_roots must be >= 0");
-    if (d.n_roots == 0) return 0;
-    GG_REQUIRE(d.n_node > 0 && d.emb && d.bias && d.indptr && d.adj && d.roots && d.tree_bits, "null graph/embedding pointer");
-    GG_REQUIRE(d.tree_words > 0, "tree_words missing (gg_tree_words)");
-    GG_REQUIRE(d.n_roots * d.n_node < (1ll << 31), "n_roots * n_node must be below 2^31 (process the roots in chunks)");
-    GG_REQUIRE(!d.edge_score || (d.hub_threshold > 0 && d.hub_threshold < SMEM_CAP), "hub_threshold out of range");
-    return 0;
+    return coop_launch(kern, WARPS_PER_CTA * 32, walk_smem_bytes(cpl, WARPS_PER_CTA), walk_min_ctas(cpl), args, st,
+                       "best-response");
 }
 
 }  // namespace
@@ -507,7 +398,7 @@ extern "C" int gg_best_response_grad_scratch_bytes(int64_t n_node, int64_t nnz, 
 
 extern "C" int gg_best_response(const gg_walk_desc *g, const int64_t *raw_indptr, const int32_t *mult, double *vstar,
                                 double *hit, int32_t *ok, void *scratch, int64_t scratch_bytes, void *stream) {
-    int rc = gg::br_check_desc(g);
+    int rc = gg::check_law_desc(g);
     if (rc || g->n_roots == 0) return rc;
     GG_REQUIRE(raw_indptr && mult, "null raw graph or multiplicity pointer");
     GG_REQUIRE(vstar && hit && ok && scratch, "null output or scratch pointer");
@@ -517,7 +408,7 @@ extern "C" int gg_best_response(const gg_walk_desc *g, const int64_t *raw_indptr
 extern "C" int gg_best_response_grad(const gg_walk_desc *g, const int64_t *raw_indptr, const int32_t *mult,
                                      const int32_t *rev, double *vstar, double *hit, int32_t *ok, double *acc_coef,
                                      double *acc_bias, void *scratch, int64_t scratch_bytes, void *stream) {
-    int rc = gg::br_check_desc(g);
+    int rc = gg::check_law_desc(g);
     if (rc || g->n_roots == 0) return rc;
     GG_REQUIRE(raw_indptr && mult && rev, "null raw graph, multiplicity or reverse-entry pointer");
     GG_REQUIRE(vstar && hit && ok && acc_coef && acc_bias && scratch, "null output, accumulator or scratch pointer");
@@ -531,13 +422,13 @@ extern "C" int gg_best_response_spmm(int64_t n_node, int32_t ld, const int64_t *
     GG_REQUIRE(n_node >= 0, "n_node must be >= 0");
     if (n_node == 0) return 0;
     GG_REQUIRE(indptr && adj && emb && acc_coef && acc_bias && grad_emb && grad_bias, "null pointer");
-    const long long *ip = (const long long *)indptr;
-    cudaStream_t st = (cudaStream_t)stream;
-    switch (ld / 32) {
-        case 1: return gg::launch_spmm<1>(n_node, ip, adj, emb, acc_coef, acc_bias, grad_emb, grad_bias, st);
-        case 2: return gg::launch_spmm<2>(n_node, ip, adj, emb, acc_coef, acc_bias, grad_emb, grad_bias, st);
-        case 4: return gg::launch_spmm<4>(n_node, ip, adj, emb, acc_coef, acc_bias, grad_emb, grad_bias, st);
-        case 8: return gg::launch_spmm<8>(n_node, ip, adj, emb, acc_coef, acc_bias, grad_emb, grad_bias, st);
-        default: return gg::launch_spmm<16>(n_node, ip, adj, emb, acc_coef, acc_bias, grad_emb, grad_bias, st);
-    }
+    return gg::with_cpl(ld, [&](auto c) {
+        unsigned grid = 0;
+        int rc = gg::fill_grid((const void *)gg::best_response_spmm_kernel<c>, 256, 0, (n_node + 7) / 8, "best-response SpMM",
+                               &grid);
+        if (rc) return rc;
+        gg::best_response_spmm_kernel<c><<<grid, 256, 0, (cudaStream_t)stream>>>(n_node, (const long long *)indptr, adj, emb,
+                                                                                 acc_coef, acc_bias, grad_emb, grad_bias);
+        return gg::check_cuda(cudaGetLastError(), "best-response SpMM launch");
+    });
 }

@@ -16,8 +16,7 @@
 //        then the same warp and CTA combination.
 #include <math.h>
 
-#include "gg_common.cuh"
-#include "value_grad.cuh"
+#include "exact.cuh"
 
 namespace gg {
 namespace {
@@ -226,6 +225,20 @@ __device__ void neg_item(const ValArgs &a, int rt, long long t, const float *s_r
     }
 }
 
+// s_root = the embedding rows of root tile rt (zero rows past the last root), between two CTA barriers
+template <int CPL>
+__device__ __forceinline__ void stage_root_tile(const ValArgs &a, long long rt, float *s_root) {
+    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
+    __syncthreads();
+    for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
+        const long long k = rt * RT + i / (LD / 4);
+        float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
+        reinterpret_cast<float4 *>(s_root)[i] = x;
+    }
+    __syncthreads();
+}
+
 // Work items: first one pos item per root (a hub root's list is the longest single item, so it starts first), then the
 // (root tile, node tile) items of neg, node tile fastest so that a CTA keeps its root rows across items.
 template <int CPL>
@@ -243,23 +256,17 @@ __global__ void __launch_bounds__(VAL_THREADS) value_kernel(const ValArgs a) {
         }
         const long long ni = item - a.n_roots, rt = ni / a.n_tiles, t = ni % a.n_tiles;
         if (rt != cur_rt) {
-            __syncthreads();
-            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
-                const long long k = rt * RT + i / (LD / 4);
-                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
-                reinterpret_cast<float4 *>(s_root)[i] = x;
-            }
-            __syncthreads();
+            stage_root_tile<CPL>(a, rt, s_root);
             cur_rt = rt;
         }
         neg_item<CPL>(a, (int)rt, t, s_root, s_part);
     }
 }
 
-// h[k, v] for every (root, node) pair: value_kernel's neg items with a store instead of the chain
-template <int CPL>
-__global__ void __launch_bounds__(VAL_THREADS) value_h_kernel(const ValArgs a, double *__restrict__ h) {
+// value_kernel's neg items with a store of each (root, node) product instead of the chain (OUT: see neg_item)
+template <int CPL, NegOut OUT>
+__device__ __forceinline__ void neg_store_items(const ValArgs &a, double *h, const int *mult = nullptr,
+                                                const double *p_void = nullptr, const double *accept = nullptr) {
     constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
     extern __shared__ __align__(16) unsigned char val_smem[];
     float *s_root = reinterpret_cast<float *>(val_smem);
@@ -269,45 +276,24 @@ __global__ void __launch_bounds__(VAL_THREADS) value_h_kernel(const ValArgs a, d
     for (long long item = blockIdx.x; item < n_items; item += gridDim.x) {
         const long long rt = item / a.n_tiles, t = item % a.n_tiles;
         if (rt != cur_rt) {
-            __syncthreads();
-            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
-                const long long k = rt * RT + i / (LD / 4);
-                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
-                reinterpret_cast<float4 *>(s_root)[i] = x;
-            }
-            __syncthreads();
+            stage_root_tile<CPL>(a, rt, s_root);
             cur_rt = rt;
         }
-        neg_item<CPL, NegOut::H>(a, (int)rt, t, s_root, s_part, h);
+        neg_item<CPL, OUT>(a, (int)rt, t, s_root, s_part, h, mult, p_void, accept);
     }
 }
 
-// W[k, v] = dV_{c_k} / ds(c_k, v) for every (root, node) pair: value_kernel's neg items with a store of dgrad_w
+// h[k, v] for every (root, node) pair
+template <int CPL>
+__global__ void __launch_bounds__(VAL_THREADS) value_h_kernel(const ValArgs a, double *__restrict__ h) {
+    neg_store_items<CPL, NegOut::H>(a, h);
+}
+
+// W[k, v] = dV_{c_k} / ds(c_k, v) for every (root, node) pair
 template <int CPL>
 __global__ void __launch_bounds__(VAL_THREADS) value_w_kernel(const ValArgs a, const int *__restrict__ mult,
                                                               double *__restrict__ W) {
-    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
-    extern __shared__ __align__(16) unsigned char val_smem[];
-    float *s_root = reinterpret_cast<float *>(val_smem);
-    double *s_part = reinterpret_cast<double *>(val_smem + (size_t)RT * LD * sizeof(float));
-    const long long n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
-    long long cur_rt = -1;
-    for (long long item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const long long rt = item / a.n_tiles, t = item % a.n_tiles;
-        if (rt != cur_rt) {
-            __syncthreads();
-            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
-                const long long k = rt * RT + i / (LD / 4);
-                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
-                reinterpret_cast<float4 *>(s_root)[i] = x;
-            }
-            __syncthreads();
-            cur_rt = rt;
-        }
-        neg_item<CPL, NegOut::W>(a, (int)rt, t, s_root, s_part, W, mult);
-    }
+    neg_store_items<CPL, NegOut::W>(a, W, mult);
 }
 
 // W_ref[k, v] for every (root, node) pair (DESIGN.md section 5.7): value_w_kernel with the D-mode law and the acceptance
@@ -315,27 +301,7 @@ template <int CPL>
 __global__ void __launch_bounds__(VAL_THREADS) value_wref_kernel(const ValArgs a, const int *__restrict__ mult,
                                                                  const double *__restrict__ p_void,
                                                                  const double *__restrict__ accept, double *__restrict__ W) {
-    constexpr int LD = 32 * CPL, RT = val_root_tile(CPL);
-    extern __shared__ __align__(16) unsigned char val_smem[];
-    float *s_root = reinterpret_cast<float *>(val_smem);
-    double *s_part = reinterpret_cast<double *>(val_smem + (size_t)RT * LD * sizeof(float));
-    const long long n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
-    long long cur_rt = -1;
-    for (long long item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const long long rt = item / a.n_tiles, t = item % a.n_tiles;
-        if (rt != cur_rt) {
-            __syncthreads();
-            for (int i = threadIdx.x; i < RT * LD / 4; i += VAL_THREADS) {
-                const long long k = rt * RT + i / (LD / 4);
-                float4 x = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-                if (k < a.n_roots) x = ldg4(a.emb + (size_t)__ldg(a.roots + k) * LD + 4 * (i % (LD / 4)));
-                reinterpret_cast<float4 *>(s_root)[i] = x;
-            }
-            __syncthreads();
-            cur_rt = rt;
-        }
-        neg_item<CPL, NegOut::WRef>(a, (int)rt, t, s_root, s_part, W, mult, p_void, accept);
-    }
+    neg_store_items<CPL, NegOut::WRef>(a, W, mult, p_void, accept);
 }
 
 // neg_c = -(sum of the root's tile partials); warp per root
@@ -356,60 +322,26 @@ __global__ void __launch_bounds__(256) value_reduce_kernel(const ValArgs a, doub
     }
 }
 
-template <int CPL>
-int launch_value(const ValArgs &a, double *neg, int *ok, cudaStream_t st) {
+// value_kernel (with_pos: its pos items first) or one of its store variants, over a grid that fills the device
+template <int CPL, class K, class... A>
+int launch_value(K kern, const ValArgs &a, bool with_pos, const char *what, cudaStream_t st, A... args) {
     const size_t smem = val_smem_bytes(CPL);
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_kernel<CPL>, VAL_THREADS, smem));
-    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
     const long long RT = val_root_tile(CPL);
-    const long long n_items = a.n_roots + (a.n_roots + RT - 1) / RT * a.n_tiles;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > n_items) grid = n_items;
-    value_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a);
-    GG_CHECK(cudaGetLastError());
-    value_reduce_kernel<<<(unsigned)((a.n_roots + 7) / 8), 256, 0, st>>>(a, neg, ok);
-    return check_cuda(cudaGetLastError(), "game value reduce launch");
+    const long long n_items = (with_pos ? a.n_roots : 0) + (a.n_roots + RT - 1) / RT * a.n_tiles;
+    unsigned grid = 0;
+    int rc = fill_grid((const void *)kern, VAL_THREADS, smem, n_items, "game value", &grid);
+    if (rc) return rc;
+    kern<<<grid, VAL_THREADS, smem, st>>>(a, args...);
+    return check_cuda(cudaGetLastError(), what);
 }
 
-template <int CPL>
-int launch_value_h(const ValArgs &a, double *h, cudaStream_t st) {
-    const size_t smem = val_smem_bytes(CPL);
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_h_kernel<CPL>, VAL_THREADS, smem));
-    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
-    const long long RT = val_root_tile(CPL), n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > n_items) grid = n_items;
-    value_h_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a, h);
-    return check_cuda(cudaGetLastError(), "game value h launch");
-}
-
-template <int CPL>
-int launch_value_w(const ValArgs &a, const int *mult, double *W, cudaStream_t st) {
-    const size_t smem = val_smem_bytes(CPL);
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_w_kernel<CPL>, VAL_THREADS, smem));
-    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
-    const long long RT = val_root_tile(CPL), n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > n_items) grid = n_items;
-    value_w_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a, mult, W);
-    return check_cuda(cudaGetLastError(), "game value W launch");
-}
-
-template <int CPL>
-int launch_value_wref(const ValArgs &a, const int *mult, const double *p_void, const double *accept, double *W,
-                      cudaStream_t st) {
-    const size_t smem = val_smem_bytes(CPL);
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, value_wref_kernel<CPL>, VAL_THREADS, smem));
-    GG_REQUIRE(per_sm >= 1, "game value kernel does not fit on an SM");
-    const long long RT = val_root_tile(CPL), n_items = (a.n_roots + RT - 1) / RT * a.n_tiles;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > n_items) grid = n_items;
-    value_wref_kernel<CPL><<<(unsigned)grid, VAL_THREADS, smem, st>>>(a, mult, p_void, accept, W);
-    return check_cuda(cudaGetLastError(), "expected D step W launch");
+// the ValArgs of the store variants
+ValArgs store_args(long long n_node, const float *emb, const float *bias, const long long *raw_indptr, long long n_roots,
+                   const int *roots, const double *dist, const int *root_ok) {
+    ValArgs a = {};
+    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = val_tiles(n_node);
+    a.emb = emb; a.bias = bias; a.raw_indptr = raw_indptr; a.roots = roots; a.dist = dist; a.root_ok = root_ok;
+    return a;
 }
 
 }  // namespace
@@ -418,47 +350,27 @@ int value_wref_launch(long long n_node, int ld, const float *emb, const float *b
                       long long n_roots, const int *roots, const double *dist_d, const double *p_void, const int *ok_ref,
                       const double *accept, const int *mult, double *W, cudaStream_t st) {
     if (n_roots == 0) return 0;
-    ValArgs a = {};
-    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = val_tiles(n_node);
-    a.emb = emb; a.bias = bias; a.raw_indptr = raw_indptr; a.roots = roots; a.dist = dist_d; a.root_ok = ok_ref;
-    switch (ld / 32) {
-        case 1: return launch_value_wref<1>(a, mult, p_void, accept, W, st);
-        case 2: return launch_value_wref<2>(a, mult, p_void, accept, W, st);
-        case 4: return launch_value_wref<4>(a, mult, p_void, accept, W, st);
-        case 8: return launch_value_wref<8>(a, mult, p_void, accept, W, st);
-        default: return launch_value_wref<16>(a, mult, p_void, accept, W, st);
-    }
+    const ValArgs a = store_args(n_node, emb, bias, raw_indptr, n_roots, roots, dist_d, ok_ref);
+    return with_cpl(ld, [&](auto c) {
+        return launch_value<c>(value_wref_kernel<c>, a, false, "expected D step W launch", st, mult, p_void, accept, W);
+    });
 }
 
 int value_w_launch(long long n_node, int ld, const float *emb, const float *bias, const long long *raw_indptr,
                    long long n_roots, const int *roots, const double *dist, const int *root_ok, const int *mult, double *W,
                    cudaStream_t st) {
     if (n_roots == 0) return 0;
-    ValArgs a = {};
-    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = val_tiles(n_node);
-    a.emb = emb; a.bias = bias; a.raw_indptr = raw_indptr; a.roots = roots; a.dist = dist; a.root_ok = root_ok;
-    switch (ld / 32) {
-        case 1: return launch_value_w<1>(a, mult, W, st);
-        case 2: return launch_value_w<2>(a, mult, W, st);
-        case 4: return launch_value_w<4>(a, mult, W, st);
-        case 8: return launch_value_w<8>(a, mult, W, st);
-        default: return launch_value_w<16>(a, mult, W, st);
-    }
+    const ValArgs a = store_args(n_node, emb, bias, raw_indptr, n_roots, roots, dist, root_ok);
+    return with_cpl(ld, [&](auto c) {
+        return launch_value<c>(value_w_kernel<c>, a, false, "game value W launch", st, mult, W);
+    });
 }
 
 int value_h_launch(long long n_node, int ld, const float *emb, const float *bias, long long n_roots, const int *roots,
                    const double *dist, double *h, cudaStream_t st) {
     if (n_roots == 0) return 0;
-    ValArgs a = {};
-    a.n_node = n_node; a.n_roots = n_roots; a.n_tiles = val_tiles(n_node);
-    a.emb = emb; a.bias = bias; a.roots = roots; a.dist = dist;
-    switch (ld / 32) {
-        case 1: return launch_value_h<1>(a, h, st);
-        case 2: return launch_value_h<2>(a, h, st);
-        case 4: return launch_value_h<4>(a, h, st);
-        case 8: return launch_value_h<8>(a, h, st);
-        default: return launch_value_h<16>(a, h, st);
-    }
+    const ValArgs a = store_args(n_node, emb, bias, nullptr, n_roots, roots, dist, nullptr);
+    return with_cpl(ld, [&](auto c) { return launch_value<c>(value_h_kernel<c>, a, false, "game value h launch", st, h); });
 }
 
 }  // namespace gg
@@ -488,11 +400,10 @@ extern "C" int gg_game_value(int64_t n_node, int32_t ld, const float *emb, const
     a.emb = emb; a.bias = bias; a.raw_indptr = (const long long *)raw_indptr; a.raw_adj = raw_adj; a.roots = roots;
     a.root_ok = root_ok; a.dist = dist; a.pos = pos; a.partial = static_cast<double *>(scratch);
     cudaStream_t st = (cudaStream_t)stream;
-    switch (ld / 32) {
-        case 1: return gg::launch_value<1>(a, neg, ok, st);
-        case 2: return gg::launch_value<2>(a, neg, ok, st);
-        case 4: return gg::launch_value<4>(a, neg, ok, st);
-        case 8: return gg::launch_value<8>(a, neg, ok, st);
-        default: return gg::launch_value<16>(a, neg, ok, st);
-    }
+    const int rc = gg::with_cpl(ld, [&](auto c) {
+        return gg::launch_value<c>(gg::value_kernel<c>, a, true, "game value launch", st);
+    });
+    if (rc) return rc;
+    gg::value_reduce_kernel<<<(unsigned)((n_roots + 7) / 8), 256, 0, st>>>(a, neg, ok);
+    return gg::check_cuda(cudaGetLastError(), "game value reduce launch");
 }

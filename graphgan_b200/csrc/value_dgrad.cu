@@ -17,7 +17,7 @@
 //
 // The expected reference D step of one pass (gg_expected_d_grad, DESIGN.md section 5.7) runs the same passes with
 // W_ref (value.cu's WRef store) in place of W and ok_ref in place of ok, after accept_kernel has formed P_acc and ok_ref.
-#include "value_grad.cuh"
+#include "exact.cuh"
 
 namespace gg {
 namespace {
@@ -207,58 +207,42 @@ __global__ void __launch_bounds__(256) accept_kernel(long long n_roots, const lo
 
 template <int CPL>
 int launch_passes(const DgArgs &a, cudaStream_t st) {
-    {
-        int per_sm = 0;
-        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cen_kernel<CPL>, DG_THREADS, 0));
-        GG_REQUIRE(per_sm >= 1, "discriminator gradient centre kernel does not fit on an SM");
-        constexpr long long CRT = 8 * cen_rw(CPL);
-        const long long n_items = (a.n_roots + CRT - 1) / CRT * a.n_ctiles;
-        long long grid = (long long)sm_count() * per_sm;
-        if (grid > n_items) grid = n_items;
-        cen_kernel<CPL><<<(unsigned)grid, DG_THREADS, 0, st>>>(a);
-        GG_CHECK(cudaGetLastError());
-        const long long n = a.n_roots * 32 * CPL;
-        cen_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, 32 * CPL);
-        GG_CHECK(cudaGetLastError());
-    }
+    constexpr long long CRT = 8 * cen_rw(CPL), NB = 8 * node_npw(CPL);
+    unsigned grid = 0;
+    int rc = fill_grid((const void *)cen_kernel<CPL>, DG_THREADS, 0, (a.n_roots + CRT - 1) / CRT * a.n_ctiles,
+                       "discriminator gradient centre", &grid);
+    if (rc) return rc;
+    cen_kernel<CPL><<<grid, DG_THREADS, 0, st>>>(a);
+    GG_CHECK(cudaGetLastError());
+    const long long n = a.n_roots * 32 * CPL;
+    cen_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a, 32 * CPL);
+    GG_CHECK(cudaGetLastError());
     const size_t smem = node_smem_bytes(CPL);
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, node_kernel<CPL>, DG_THREADS, smem));
-    GG_REQUIRE(per_sm >= 1, "discriminator gradient node kernel does not fit on an SM");
-    const long long n_items = (a.n_node + 8 * node_npw(CPL) - 1) / (8 * node_npw(CPL));
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > n_items) grid = n_items;
-    node_kernel<CPL><<<(unsigned)grid, DG_THREADS, smem, st>>>(a);
+    rc = fill_grid((const void *)node_kernel<CPL>, DG_THREADS, smem, (a.n_node + NB - 1) / NB, "discriminator gradient node",
+                   &grid);
+    if (rc) return rc;
+    node_kernel<CPL><<<grid, DG_THREADS, smem, st>>>(a);
     return check_cuda(cudaGetLastError(), "discriminator gradient node launch");
 }
 
 struct DgLayout {
     int *mult;
     double *W, *partial, *C;
+    int *ok_ref;                                // gg_expected_d_grad only
 };
 
-size_t dg_layout(void *buf, long long n_node, int ld, long long n_roots, DgLayout *v) {
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
+// gg_game_value_grad_d's scratch; with ok_ref (gg_expected_d_grad), then ok_ref [n_roots]
+size_t dg_layout(void *buf, long long n_node, int ld, long long n_roots, bool ok_ref, DgLayout *v) {
     const size_t rn = (size_t)n_roots * (size_t)n_node;
-    const size_t o_m = take(rn * sizeof(int)), o_w = take(rn * sizeof(double));
-    const size_t o_p = take((size_t)n_roots * (size_t)cen_tiles(n_node) * (size_t)ld * sizeof(double));
-    const size_t o_c = take((size_t)n_roots * (size_t)ld * sizeof(double));
-    if (buf && v) {
-        unsigned char *b = static_cast<unsigned char *>(buf);
-        v->mult = reinterpret_cast<int *>(b + o_m);
-        v->W = reinterpret_cast<double *>(b + o_w);
-        v->partial = reinterpret_cast<double *>(b + o_p);
-        v->C = reinterpret_cast<double *>(b + o_c);
-    }
-    return off;
-}
-
-// gg_expected_d_grad's scratch: dg_layout, then ok_ref [n_roots]
-size_t dref_layout(void *buf, long long n_node, int ld, long long n_roots, DgLayout *v, int **ok_ref) {
-    const size_t off = dg_layout(buf, n_node, ld, n_roots, v);
-    if (buf && ok_ref) *ok_ref = reinterpret_cast<int *>(static_cast<unsigned char *>(buf) + off);
-    return off + (((size_t)n_roots * sizeof(int) + 255) & ~(size_t)255);
+    Slab s(buf);
+    DgLayout t;
+    t.mult = s.take<int>(rn);
+    t.W = s.take<double>(rn);
+    t.partial = s.take<double>((size_t)n_roots * (size_t)cen_tiles(n_node) * (size_t)ld);
+    t.C = s.take<double>((size_t)n_roots * (size_t)ld);
+    t.ok_ref = ok_ref ? s.take<int>((size_t)n_roots) : nullptr;
+    if (buf && v) *v = t;
+    return s.off;
 }
 
 }  // namespace
@@ -267,7 +251,7 @@ size_t dref_layout(void *buf, long long n_node, int ld, long long n_roots, DgLay
 extern "C" int gg_game_value_grad_d_scratch_bytes(int64_t n_node, int32_t ld, int64_t n_roots, int64_t *bytes) {
     GG_REQUIRE(bytes && n_node >= 0 && n_roots >= 0, "bad arguments");
     GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
-    *bytes = (int64_t)gg::dg_layout(nullptr, n_node, ld, n_roots, nullptr);
+    *bytes = (int64_t)gg::dg_layout(nullptr, n_node, ld, n_roots, false, nullptr);
     return 0;
 }
 
@@ -283,7 +267,7 @@ extern "C" int gg_game_value_grad_d(int64_t n_node, int32_t ld, const float *emb
     GG_REQUIRE(dist && root_ok, "null generator distribution pointer");
     GG_REQUIRE(grad_emb && grad_bias && scratch, "null output or scratch pointer");
     gg::DgLayout v;
-    const size_t need = gg::dg_layout(scratch, n_node, ld, n_roots, &v);
+    const size_t need = gg::dg_layout(scratch, n_node, ld, n_roots, false, &v);
     GG_REQUIRE(scratch_bytes >= (int64_t)need, "scratch too small (gg_game_value_grad_d_scratch_bytes)");
     cudaStream_t st = (cudaStream_t)stream;
     gg::DgArgs a;
@@ -295,19 +279,13 @@ extern "C" int gg_game_value_grad_d(int64_t n_node, int32_t ld, const float *emb
     GG_CHECK(cudaGetLastError());
     int rc = gg::value_w_launch(n_node, ld, emb, bias, a.raw_indptr, n_roots, roots, dist, root_ok, v.mult, v.W, st);
     if (rc) return rc;
-    switch (ld / 32) {
-        case 1: return gg::launch_passes<1>(a, st);
-        case 2: return gg::launch_passes<2>(a, st);
-        case 4: return gg::launch_passes<4>(a, st);
-        case 8: return gg::launch_passes<8>(a, st);
-        default: return gg::launch_passes<16>(a, st);
-    }
+    return gg::with_cpl(ld, [&](auto c) { return gg::launch_passes<c>(a, st); });
 }
 
 extern "C" int gg_expected_d_grad_scratch_bytes(int64_t n_node, int32_t ld, int64_t n_roots, int64_t *bytes) {
     GG_REQUIRE(bytes && n_node >= 0 && n_roots >= 0, "bad arguments");
     GG_REQUIRE(gg::ld_supported(ld), GG_LD_MESSAGE);
-    *bytes = (int64_t)gg::dref_layout(nullptr, n_node, ld, n_roots, nullptr, nullptr);
+    *bytes = (int64_t)gg::dg_layout(nullptr, n_node, ld, n_roots, true, nullptr);
     return 0;
 }
 
@@ -323,8 +301,8 @@ extern "C" int gg_expected_d_grad(int64_t n_node, int32_t ld, const float *emb, 
     GG_REQUIRE(dist_d && p_void && root_ok, "null D-mode law pointer");
     GG_REQUIRE(accept && grad_emb && grad_bias && scratch, "null output or scratch pointer");
     gg::DgLayout v;
-    int *ok_ref = nullptr;
-    const size_t need = gg::dref_layout(scratch, n_node, ld, n_roots, &v, &ok_ref);
+    const size_t need = gg::dg_layout(scratch, n_node, ld, n_roots, true, &v);
+    int *ok_ref = v.ok_ref;
     GG_REQUIRE(scratch_bytes >= (int64_t)need, "scratch too small (gg_expected_d_grad_scratch_bytes)");
     cudaStream_t st = (cudaStream_t)stream;
     const long long *rip = (const long long *)raw_indptr;
@@ -339,11 +317,5 @@ extern "C" int gg_expected_d_grad(int64_t n_node, int32_t ld, const float *emb, 
     GG_CHECK(cudaGetLastError());
     int rc = gg::value_wref_launch(n_node, ld, emb, bias, rip, n_roots, roots, dist_d, p_void, ok_ref, accept, v.mult, v.W, st);
     if (rc) return rc;
-    switch (ld / 32) {
-        case 1: return gg::launch_passes<1>(a, st);
-        case 2: return gg::launch_passes<2>(a, st);
-        case 4: return gg::launch_passes<4>(a, st);
-        case 8: return gg::launch_passes<8>(a, st);
-        default: return gg::launch_passes<16>(a, st);
-    }
+    return gg::with_cpl(ld, [&](auto c) { return gg::launch_passes<c>(a, st); });
 }

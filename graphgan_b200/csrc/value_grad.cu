@@ -22,8 +22,7 @@
 #include <cooperative_groups.h>
 #include <math.h>
 
-#include "value_grad.cuh"
-#include "walk_common.cuh"
+#include "exact.cuh"
 
 namespace gg {
 namespace {
@@ -32,7 +31,6 @@ namespace cg = cooperative_groups;
 
 constexpr int VG_THREADS = 256;
 constexpr int VG_CHAINS = VG_THREADS / 32;     // 8 chains, one per warp of a hub node's CTA
-constexpr long long VG_BLOCK = 256;            // entries per chain block; lists up to this length are one warp's item
 
 struct VgArgs {
     long long n_node, n_roots, tree_words;
@@ -46,18 +44,10 @@ struct VgArgs {
     const int *father;
     const int4 *items;
     const unsigned *lev_off, *n_lev;
-    int *big;                                  // [n_node]: nodes with more than VG_BLOCK entries; big_cnt: their number
+    int *big;                                  // [n_node]: nodes with more than CHAIN_BLOCK entries; big_cnt: their number
     unsigned *big_cnt;
     double *grad_emb, *grad_bias;
 };
-
-__device__ __forceinline__ bool tree_bit(const uint32_t *tb, long long e) { return (__ldg(tb + (e >> 5)) >> (e & 31)) & 1u; }
-
-__device__ __forceinline__ double warp_dsum(double x) {
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) x = __dadd_rn(x, __shfl_xor_sync(FULL, x, off));
-    return x;
-}
 
 // one item (slot, a) of the bottom-up pass: T(a), then (w_in, w_stop) of a's reached children
 __device__ void tsum_item(const VgArgs &g, const int4 it, int lane) {
@@ -96,13 +86,6 @@ __global__ void __launch_bounds__(VG_THREADS) tsum_kernel(const VgArgs g) {
     }
 }
 
-// the nodes with more than VG_BLOCK entries, in any order (each is one independent item)
-__global__ void big_nodes_kernel(const VgArgs g) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= g.n_node) return;
-    if (__ldg(g.indptr + i + 1) - __ldg(g.indptr + i) > VG_BLOCK) g.big[atomicAdd(g.big_cnt, 1u)] = (int)i;
-}
-
 // chain_q of node a in root slot k (see the top of the file): s[i] for coordinate lane + 32 i, sb for the bias.  The
 // children's (x, c_e, w_x(a)) are broadcast from the lanes that found them; four rows are in flight.
 template <int CPL>
@@ -112,8 +95,8 @@ __device__ __forceinline__ void child_chain(const VgArgs &g, size_t o, const uin
 #pragma unroll
     for (int i = 0; i < CPL; ++i) s[i] = 0.0;
     sb = 0.0;
-    for (long long b0 = a0 + VG_BLOCK * q; b0 < a1; b0 += VG_BLOCK * VG_CHAINS) {
-        const long long b1 = b0 + VG_BLOCK < a1 ? b0 + VG_BLOCK : a1;
+    for (long long b0 = a0 + CHAIN_BLOCK * q; b0 < a1; b0 += CHAIN_BLOCK * VG_CHAINS) {
+        const long long b1 = b0 + CHAIN_BLOCK < a1 ? b0 + CHAIN_BLOCK : a1;
         for (long long e0 = b0; e0 < b1; e0 += 32) {
             const long long e = e0 + lane;
             int x = -1;
@@ -223,7 +206,7 @@ __global__ void __launch_bounds__(VG_THREADS) gather_kernel(const VgArgs g) {
         const long long a = (item - n_big) * VG_CHAINS + wid;
         if (a >= g.n_node) continue;
         const long long a0 = __ldg(g.indptr + a), a1 = __ldg(g.indptr + a + 1);
-        if (a1 - a0 > VG_BLOCK) continue;
+        if (a1 - a0 > CHAIN_BLOCK) continue;
         double acc[CPL];
 #pragma unroll
         for (int i = 0; i < CPL; ++i) acc[i] = g.grad_emb[(size_t)a * LD + lane + 32 * i];
@@ -251,19 +234,6 @@ __global__ void __launch_bounds__(VG_THREADS) gather_kernel(const VgArgs g) {
     }
 }
 
-template <int CPL>
-int launch_gather(const VgArgs &g, cudaStream_t st) {
-    const size_t smem = (size_t)VG_CHAINS * (32 * CPL + 1) * sizeof(double);
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gather_kernel<CPL>, VG_THREADS, smem));
-    GG_REQUIRE(per_sm >= 1, "value gradient gather kernel does not fit on an SM");
-    const long long n_groups = (g.n_node + VG_CHAINS - 1) / VG_CHAINS;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > n_groups + g.n_node) grid = n_groups + g.n_node;
-    gather_kernel<CPL><<<(unsigned)grid, VG_THREADS, smem, st>>>(g);
-    return check_cuda(cudaGetLastError(), "value gradient gather launch");
-}
-
 struct VgLayout {
     void *rec;                                 // gdist_rec_layout's part
     double *dist, *h, *T, *pi_in, *pi_stop, *partial;
@@ -273,35 +243,41 @@ struct VgLayout {
 };
 
 size_t vg_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, VgLayout *v) {
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
     const size_t rn = (size_t)n_roots * (size_t)n_node;
     int64_t partial = 0;
     gg_game_value_scratch_bytes(n_node, n_roots, &partial);
-    const size_t o_rec = take(gdist_rec_layout(nullptr, n_node, nnz_words, n_roots, nullptr));
-    const size_t o_dist = take(rn * sizeof(double)), o_h = take(rn * sizeof(double)), o_T = take(rn * sizeof(double));
-    const size_t o_pin = take(rn * sizeof(double)), o_pst = take(rn * sizeof(double));
-    const size_t o_fa = take(rn * sizeof(int)), o_ok = take((size_t)n_roots * sizeof(int));
-    const size_t o_part = take((size_t)partial), o_big = take((size_t)n_node * sizeof(int)), o_bc = take(sizeof(unsigned));
-    if (buf && v) {
-        unsigned char *b = static_cast<unsigned char *>(buf);
-        v->rec = b + o_rec;
-        v->dist = reinterpret_cast<double *>(b + o_dist);
-        v->h = reinterpret_cast<double *>(b + o_h);
-        v->T = reinterpret_cast<double *>(b + o_T);
-        v->pi_in = reinterpret_cast<double *>(b + o_pin);
-        v->pi_stop = reinterpret_cast<double *>(b + o_pst);
-        v->father = reinterpret_cast<int *>(b + o_fa);
-        v->root_ok = reinterpret_cast<int *>(b + o_ok);
-        v->partial = reinterpret_cast<double *>(b + o_part);
-        v->partial_bytes = (size_t)partial;
-        v->big = reinterpret_cast<int *>(b + o_big);
-        v->big_cnt = reinterpret_cast<unsigned *>(b + o_bc);
-    }
-    return off;
+    Slab s(buf);
+    VgLayout t;
+    t.rec = s.take<unsigned char>(gdist_rec_layout(nullptr, n_node, nnz_words, n_roots, nullptr));
+    t.dist = s.take<double>(rn);
+    t.h = s.take<double>(rn);
+    t.T = s.take<double>(rn);
+    t.pi_in = s.take<double>(rn);
+    t.pi_stop = s.take<double>(rn);
+    t.father = s.take<int>(rn);
+    t.root_ok = s.take<int>((size_t)n_roots);
+    t.partial = s.take<double>((size_t)partial / sizeof(double));
+    t.partial_bytes = (size_t)partial;
+    t.big = s.take<int>((size_t)n_node);
+    t.big_cnt = s.take<unsigned>(1);
+    if (buf && v) *v = t;
+    return s.off;
 }
 
 }  // namespace
+
+// the nodes with more than CHAIN_BLOCK entries, in any order (each is one independent item)
+__global__ void big_nodes_kernel(long long n_node, const long long *indptr, int *big, unsigned *big_cnt) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_node) return;
+    if (__ldg(indptr + i + 1) - __ldg(indptr + i) > CHAIN_BLOCK) big[atomicAdd(big_cnt, 1u)] = (int)i;
+}
+
+int big_nodes_launch(long long n_node, const long long *indptr, int *big, unsigned *big_cnt, cudaStream_t st) {
+    big_nodes_kernel<<<(unsigned)((n_node + 255) / 256), 256, 0, st>>>(n_node, indptr, big, big_cnt);
+    return check_cuda(cudaGetLastError(), "big-node list launch");
+}
+
 }  // namespace gg
 
 extern "C" int gg_game_value_grad_scratch_bytes(int64_t n_node, int64_t nnz, int64_t n_roots, int64_t *bytes) {
@@ -313,17 +289,11 @@ extern "C" int gg_game_value_grad_scratch_bytes(int64_t n_node, int64_t nnz, int
 extern "C" int gg_game_value_grad(const gg_walk_desc *gp, const float *d_emb, const float *d_bias, const int64_t *raw_indptr,
                                   const int32_t *raw_adj, double *pos, double *neg, int32_t *ok, double *grad_emb,
                                   double *grad_bias, void *scratch, int64_t scratch_bytes, void *stream) {
-    GG_REQUIRE(gp, "null descriptor");
+    int rc = gg::check_law_desc(gp);
+    if (rc || gp->n_roots == 0) return rc;
     const gg_walk_desc &d = *gp;
-    GG_REQUIRE(gg::ld_supported(d.ld), GG_LD_MESSAGE);
-    GG_REQUIRE(d.n_roots >= 0, "n_roots must be >= 0");
-    if (d.n_roots == 0) return 0;
-    GG_REQUIRE(d.n_node > 0 && d.emb && d.bias && d.indptr && d.adj && d.roots && d.tree_bits, "null graph/embedding pointer");
-    GG_REQUIRE(d.tree_words > 0, "tree_words missing (gg_tree_words)");
     GG_REQUIRE(d_emb && d_bias && raw_indptr && raw_adj, "null discriminator or raw graph pointer");
     GG_REQUIRE(pos && neg && ok && grad_emb && grad_bias && scratch, "null output or scratch pointer");
-    GG_REQUIRE(d.n_roots * d.n_node < (1ll << 31), "n_roots * n_node must be below 2^31 (process the roots in chunks)");
-    GG_REQUIRE(!d.edge_score || (d.hub_threshold > 0 && d.hub_threshold < gg::SMEM_CAP), "hub_threshold out of range");
     gg::VgLayout v;
     const size_t need = gg::vg_layout(scratch, d.n_node, d.tree_words - 1, d.n_roots, &v);
     GG_REQUIRE(scratch_bytes >= (int64_t)need, "scratch too small (gg_game_value_grad_scratch_bytes)");
@@ -338,7 +308,7 @@ extern "C" int gg_game_value_grad(const gg_walk_desc *gp, const float *d_emb, co
     gg::GdRec rec;
     rec.pi_in = v.pi_in; rec.pi_stop = v.pi_stop; rec.father = v.father;
     gg::gdist_rec_layout(v.rec, d.n_node, d.tree_words - 1, d.n_roots, &rec);
-    int rc = gg::gdist_rec_launch(d, v.dist, v.root_ok, rec, v.rec, st);
+    rc = gg::gdist_rec_launch(d, v.dist, v.root_ok, rec, v.rec, st);
     if (rc) return rc;
     rc = gg_game_value(d.n_node, d.ld, d_emb, d_bias, raw_indptr, raw_adj, d.n_roots, d.roots, v.dist, v.root_ok, pos, neg,
                        ok, v.partial, (int64_t)v.partial_bytes, stream);
@@ -351,22 +321,19 @@ extern "C" int gg_game_value_grad(const gg_walk_desc *gp, const float *d_emb, co
     g.emb = d.emb; g.h = v.h; g.T = v.T; g.w_in = v.pi_in; g.w_stop = v.pi_stop; g.father = v.father;
     g.items = rec.items; g.lev_off = rec.lev_off; g.n_lev = rec.n_lev; g.big = v.big; g.big_cnt = v.big_cnt;
     g.grad_emb = grad_emb; g.grad_bias = grad_bias;
-    {
-        int dev = 0, per_sm = 0;
-        GG_CHECK(cudaGetDevice(&dev));
-        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gg::tsum_kernel, gg::VG_THREADS, 0));
-        GG_REQUIRE(per_sm >= 1, "value gradient tsum kernel does not fit on an SM");
-        void *args[] = {(void *)&g};
-        GG_CHECK(cudaLaunchCooperativeKernel((const void *)gg::tsum_kernel, dim3((unsigned)(gg::sm_count() * per_sm)),
-                                             dim3(gg::VG_THREADS), args, 0, st));
-    }
-    gg::big_nodes_kernel<<<(unsigned)((d.n_node + 255) / 256), 256, 0, st>>>(g);
-    GG_CHECK(cudaGetLastError());
-    switch (d.ld / 32) {
-        case 1: return gg::launch_gather<1>(g, st);
-        case 2: return gg::launch_gather<2>(g, st);
-        case 4: return gg::launch_gather<4>(g, st);
-        case 8: return gg::launch_gather<8>(g, st);
-        default: return gg::launch_gather<16>(g, st);
-    }
+    void *args[] = {(void *)&g};
+    rc = gg::coop_launch((const void *)gg::tsum_kernel, gg::VG_THREADS, 0, 0, args, st, "value gradient tsum");
+    if (rc) return rc;
+    rc = gg::big_nodes_launch(d.n_node, g.indptr, v.big, v.big_cnt, st);
+    if (rc) return rc;
+    return gg::with_cpl(d.ld, [&](auto c) {
+        const size_t smem = (size_t)gg::VG_CHAINS * (32 * c + 1) * sizeof(double);
+        unsigned grid = 0;
+        const long long n_groups = (g.n_node + gg::VG_CHAINS - 1) / gg::VG_CHAINS;
+        int rc = gg::fill_grid((const void *)gg::gather_kernel<c>, gg::VG_THREADS, smem, n_groups + g.n_node,
+                               "value gradient gather", &grid);
+        if (rc) return rc;
+        gg::gather_kernel<c><<<grid, gg::VG_THREADS, smem, st>>>(g);
+        return gg::check_cuda(cudaGetLastError(), "value gradient gather launch");
+    });
 }

@@ -39,9 +39,8 @@
 #include <cooperative_groups.h>
 #include <math.h>
 
+#include "exact.cuh"
 #include "update_dev.cuh"
-#include "value_grad.cuh"
-#include "walk_common.cuh"
 
 namespace gg {
 namespace {
@@ -50,7 +49,6 @@ namespace cg = cooperative_groups;
 
 constexpr int GR_THREADS = 256;
 constexpr int GR_CHAINS = GR_THREADS / 32;     // 8 chains, one per warp of a hub node's CTA
-constexpr long long GR_BLOCK = 256;            // entries per chain block; lists up to this length are one warp's item
 constexpr int GR_WMAX = 8;                     // the largest window
 
 struct GrArgs {
@@ -70,14 +68,6 @@ struct GrArgs {
     unsigned *big_cnt;
     double *n_pairs, *grad_emb, *grad_bias;
 };
-
-__device__ __forceinline__ bool tree_bit(const uint32_t *tb, long long e) { return (__ldg(tb + (e >> 5)) >> (e & 31)) & 1u; }
-
-__device__ __forceinline__ double warp_dsum(double x) {
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) x = __dadd_rn(x, __shfl_xor_sync(FULL, x, off));
-    return x;
-}
 
 // top-down over the recorded levels, a thread per item, one grid barrier per level
 __global__ void __launch_bounds__(GR_THREADS) reach_kernel(const GrArgs g) {
@@ -168,12 +158,6 @@ __global__ void __launch_bounds__(GR_THREADS) npairs_kernel(const GrArgs g) {
     }
 }
 
-__global__ void big_nodes_kernel(const GrArgs g) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= g.n_node) return;
-    if (__ldg(g.indptr + i + 1) - __ldg(g.indptr + i) > GR_BLOCK) g.big[atomicAdd(g.big_cnt, 1u)] = (int)i;
-}
-
 // the pair coefficient c = rho (kappa_up + kappa_dn) of (anc_d(y), y) and the bias term of its node side
 __device__ __forceinline__ double pair_coef(const GrArgs &g, size_t o, int y, int d, double &rho) {
     const size_t at = (size_t)(d - 1) * (size_t)g.rn + o + y;
@@ -194,9 +178,9 @@ __device__ __forceinline__ void down_chain(const GrArgs &g, size_t o, const uint
     int nd[GR_WMAX];
     long long nxt[GR_WMAX], end[GR_WMAX], base[GR_WMAX];
     unsigned msk[GR_WMAX];
-    for (long long b0 = a0 + GR_BLOCK * q; b0 < a1; b0 += GR_BLOCK * GR_CHAINS) {
+    for (long long b0 = a0 + CHAIN_BLOCK * q; b0 < a1; b0 += CHAIN_BLOCK * GR_CHAINS) {
         int top = 0;
-        nd[0] = a; nxt[0] = b0; end[0] = b0 + GR_BLOCK < a1 ? b0 + GR_BLOCK : a1; msk[0] = 0u; base[0] = b0;
+        nd[0] = a; nxt[0] = b0; end[0] = b0 + CHAIN_BLOCK < a1 ? b0 + CHAIN_BLOCK : a1; msk[0] = 0u; base[0] = b0;
         while (true) {
             if (msk[top] == 0u) {
                 if (nxt[top] >= end[top]) {
@@ -318,7 +302,7 @@ __device__ __forceinline__ void gather_rows(const GrArgs &g, double *mnp) {
         const long long a = (item - n_big) * GR_CHAINS + wid;
         if (a >= g.n_node) continue;
         const long long a0 = __ldg(g.indptr + a), a1 = __ldg(g.indptr + a + 1);
-        if (a1 - a0 > GR_BLOCK) continue;
+        if (a1 - a0 > CHAIN_BLOCK) continue;
         double acc[CPL];
 #pragma unroll
         for (int i = 0; i < CPL; ++i) acc[i] = g.grad_emb[(size_t)a * LD + lane + 32 * i];
@@ -369,32 +353,21 @@ template <int CPL>
 __global__ void __launch_bounds__(GR_THREADS) gather_sq_kernel(const GrArgs g, double *mnp) { gather_rows<CPL, true>(g, mnp); }
 
 // gather_kernel, or gather_sq_kernel when mnp is given
-template <int CPL>
-int launch_gather(const GrArgs &g, double *mnp, cudaStream_t st) {
-    const size_t smem = (size_t)GR_CHAINS * (32 * CPL + (mnp ? 2 : 1)) * sizeof(double);
-    const void *fn = mnp ? (const void *)gather_sq_kernel<CPL> : (const void *)gather_kernel<CPL>;
-    GG_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, GR_THREADS, smem));
-    GG_REQUIRE(per_sm >= 1, "expected G step gather kernel does not fit on an SM");
-    const long long n_groups = (g.n_node + GR_CHAINS - 1) / GR_CHAINS;
-    long long grid = (long long)sm_count() * per_sm;
-    if (grid > n_groups + g.n_node) grid = n_groups + g.n_node;
-    if (mnp)
-        gather_sq_kernel<CPL><<<(unsigned)grid, GR_THREADS, smem, st>>>(g, mnp);
-    else
-        gather_kernel<CPL><<<(unsigned)grid, GR_THREADS, smem, st>>>(g);
-    return check_cuda(cudaGetLastError(), "expected G step gather launch");
-}
-
 int gather(const GrArgs &g, double *mnp, cudaStream_t st) {
-    switch (g.ld / 32) {
-        case 1: return launch_gather<1>(g, mnp, st);
-        case 2: return launch_gather<2>(g, mnp, st);
-        case 4: return launch_gather<4>(g, mnp, st);
-        case 8: return launch_gather<8>(g, mnp, st);
-        default: return launch_gather<16>(g, mnp, st);
-    }
+    return with_cpl(g.ld, [&](auto c) {
+        const size_t smem = (size_t)GR_CHAINS * (32 * c + (mnp ? 2 : 1)) * sizeof(double);
+        const void *fn = mnp ? (const void *)gather_sq_kernel<c> : (const void *)gather_kernel<c>;
+        GG_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const long long n_groups = (g.n_node + GR_CHAINS - 1) / GR_CHAINS;
+        unsigned grid = 0;
+        int rc = fill_grid(fn, GR_THREADS, smem, n_groups + g.n_node, "expected G step gather", &grid);
+        if (rc) return rc;
+        if (mnp)
+            gather_sq_kernel<c><<<grid, GR_THREADS, smem, st>>>(g, mnp);
+        else
+            gather_kernel<c><<<grid, GR_THREADS, smem, st>>>(g);
+        return check_cuda(cudaGetLastError(), "expected G step gather launch");
+    });
 }
 
 // ---- section 5.9: the second moment of one walk's step
@@ -523,33 +496,24 @@ struct GrLayout {
 };
 
 size_t gr_layout(void *buf, long long n_node, long long nnz_words, long long n_roots, int window, bool moments, GrLayout *v) {
-    size_t off = 0;
-    auto take = [&](size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; };
     const size_t rn = (size_t)n_roots * (size_t)n_node;
-    const size_t o_rec = take(gdist_rec_layout(nullptr, n_node, nnz_words, n_roots, nullptr));
-    const size_t o_dist = take(rn * sizeof(double)), o_reach = take(rn * sizeof(double));
-    const size_t o_pin = take(rn * sizeof(double)), o_pst = take(rn * sizeof(double));
-    const size_t o_kup = take((size_t)window * rn * sizeof(float)), o_kdn = take((size_t)window * rn * sizeof(float));
-    const size_t o_fa = take(rn * sizeof(int)), o_ok = take((size_t)n_roots * sizeof(int));
-    const size_t o_big = take((size_t)n_node * sizeof(int)), o_bc = take(sizeof(unsigned));
-    const size_t o_pf = moments ? take(rn * sizeof(double)) : 0, o_sqn = moments ? take(rn * sizeof(double)) : 0;
-    if (buf && v) {
-        unsigned char *b = static_cast<unsigned char *>(buf);
-        v->rec = b + o_rec;
-        v->dist = reinterpret_cast<double *>(b + o_dist);
-        v->reach = reinterpret_cast<double *>(b + o_reach);
-        v->pi_in = reinterpret_cast<double *>(b + o_pin);
-        v->pi_stop = reinterpret_cast<double *>(b + o_pst);
-        v->kup = reinterpret_cast<float *>(b + o_kup);
-        v->kdn = reinterpret_cast<float *>(b + o_kdn);
-        v->father = reinterpret_cast<int *>(b + o_fa);
-        v->root_ok = reinterpret_cast<int *>(b + o_ok);
-        v->big = reinterpret_cast<int *>(b + o_big);
-        v->big_cnt = reinterpret_cast<unsigned *>(b + o_bc);
-        v->pf = moments ? reinterpret_cast<double *>(b + o_pf) : nullptr;
-        v->sqn = moments ? reinterpret_cast<double *>(b + o_sqn) : nullptr;
-    }
-    return off;
+    Slab s(buf);
+    GrLayout t;
+    t.rec = s.take<unsigned char>(gdist_rec_layout(nullptr, n_node, nnz_words, n_roots, nullptr));
+    t.dist = s.take<double>(rn);
+    t.reach = s.take<double>(rn);
+    t.pi_in = s.take<double>(rn);
+    t.pi_stop = s.take<double>(rn);
+    t.kup = s.take<float>((size_t)window * rn);
+    t.kdn = s.take<float>((size_t)window * rn);
+    t.father = s.take<int>(rn);
+    t.root_ok = s.take<int>((size_t)n_roots);
+    t.big = s.take<int>((size_t)n_node);
+    t.big_cnt = s.take<unsigned>(1);
+    t.pf = moments ? s.take<double>(rn) : nullptr;
+    t.sqn = moments ? s.take<double>(rn) : nullptr;
+    if (buf && v) *v = t;
+    return s.off;
 }
 
 struct GmOut {
@@ -560,19 +524,13 @@ struct GmOut {
 int expected_g_run(const gg_walk_desc *gp, const float *d_emb, const float *d_bias, int32_t window, double *n_pairs,
                    int32_t *root_ok, double *grad_emb, double *grad_bias, void *scratch, int64_t scratch_bytes, void *stream,
                    const GmOut *mo) {
-    GG_REQUIRE(gp, "null descriptor");
-    const gg_walk_desc &d = *gp;
-    GG_REQUIRE(ld_supported(d.ld), GG_LD_MESSAGE);
     GG_REQUIRE(window >= 1 && window <= GR_WMAX, "window must be 1 .. 8");
-    GG_REQUIRE(d.n_roots >= 0, "n_roots must be >= 0");
-    if (d.n_roots == 0) return 0;
-    GG_REQUIRE(d.n_node > 0 && d.emb && d.bias && d.indptr && d.adj && d.roots && d.tree_bits, "null graph/embedding pointer");
-    GG_REQUIRE(d.tree_words > 0, "tree_words missing (gg_tree_words)");
+    int rc = check_law_desc(gp);
+    if (rc || gp->n_roots == 0) return rc;
+    const gg_walk_desc &d = *gp;
     GG_REQUIRE(d_emb && d_bias, "null discriminator pointer");
     GG_REQUIRE(n_pairs && root_ok && grad_emb && grad_bias && scratch, "null output or scratch pointer");
     GG_REQUIRE(!mo || (mo->sq && mo->mn), "null sq / mn pointer");
-    GG_REQUIRE(d.n_roots * d.n_node < (1ll << 31), "n_roots * n_node must be below 2^31 (process the roots in chunks)");
-    GG_REQUIRE(!d.edge_score || (d.hub_threshold > 0 && d.hub_threshold < SMEM_CAP), "hub_threshold out of range");
     GrLayout v;
     const size_t need = gr_layout(scratch, d.n_node, d.tree_words - 1, d.n_roots, window, mo != nullptr, &v);
     GG_REQUIRE(scratch_bytes >= (int64_t)need, mo ? "scratch too small (gg_expected_g_moments_scratch_bytes)"
@@ -586,7 +544,7 @@ int expected_g_run(const gg_walk_desc *gp, const float *d_emb, const float *d_bi
     GdRec rec;
     rec.pi_in = v.pi_in; rec.pi_stop = v.pi_stop; rec.father = v.father;
     gdist_rec_layout(v.rec, d.n_node, d.tree_words - 1, d.n_roots, &rec);
-    int rc = gdist_rec_launch(d, v.dist, root_ok, rec, v.rec, st);
+    rc = gdist_rec_launch(d, v.dist, root_ok, rec, v.rec, st);
     if (rc) return rc;
     GrArgs g;
     g.n_node = d.n_node; g.n_roots = d.n_roots; g.tree_words = d.tree_words; g.rn = (long long)rn;
@@ -597,21 +555,16 @@ int expected_g_run(const gg_walk_desc *gp, const float *d_emb, const float *d_bi
     g.items = rec.items; g.lev_off = rec.lev_off; g.n_lev = rec.n_lev;
     g.kup = v.kup; g.kdn = v.kdn; g.big = v.big; g.big_cnt = v.big_cnt;
     g.n_pairs = n_pairs; g.grad_emb = grad_emb; g.grad_bias = grad_bias;
-    {
-        int per_sm = 0;
-        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, reach_kernel, GR_THREADS, 0));
-        GG_REQUIRE(per_sm >= 1, "expected G step reach kernel does not fit on an SM");
-        void *args[] = {(void *)&g};
-        GG_CHECK(cudaLaunchCooperativeKernel((const void *)reach_kernel, dim3((unsigned)(sm_count() * per_sm)),
-                                             dim3(GR_THREADS), args, 0, st));
-    }
+    void *args[] = {(void *)&g};
+    rc = coop_launch((const void *)reach_kernel, GR_THREADS, 0, 0, args, st, "expected G step reach");
+    if (rc) return rc;
     score_kernel<<<(unsigned)(sm_count() * 8), GR_THREADS, 0, st>>>(g);
     GG_CHECK(cudaGetLastError());
     const unsigned root_grid = (unsigned)(d.n_roots < sm_count() * 4 ? d.n_roots : sm_count() * 4);
     npairs_kernel<<<root_grid, GR_THREADS, 0, st>>>(g);
     GG_CHECK(cudaGetLastError());
-    big_nodes_kernel<<<(unsigned)((d.n_node + 255) / 256), 256, 0, st>>>(g);
-    GG_CHECK(cudaGetLastError());
+    rc = big_nodes_launch(d.n_node, g.indptr, v.big, v.big_cnt, st);
+    if (rc) return rc;
     if (!mo) return gather(g, nullptr, st);
     GmArgs m;
     m.g = g; m.dist = v.dist; m.pf = v.pf; m.sqn = mo->sq_node ? mo->sq_node : v.sqn;
@@ -619,14 +572,9 @@ int expected_g_run(const gg_walk_desc *gp, const float *d_emb, const float *d_bi
     GG_CHECK(cudaMemsetAsync(m.sqn, 0, rn * sizeof(double), st));
     moment_kernel<<<(unsigned)(sm_count() * 8), GR_THREADS, 0, st>>>(m);
     GG_CHECK(cudaGetLastError());
-    {
-        int per_sm = 0;
-        GG_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, moment_prefix_kernel, GR_THREADS, 0));
-        GG_REQUIRE(per_sm >= 1, "expected G moments prefix kernel does not fit on an SM");
-        void *args[] = {(void *)&m};
-        GG_CHECK(cudaLaunchCooperativeKernel((const void *)moment_prefix_kernel, dim3((unsigned)(sm_count() * per_sm)),
-                                             dim3(GR_THREADS), args, 0, st));
-    }
+    void *margs[] = {(void *)&m};
+    rc = coop_launch((const void *)moment_prefix_kernel, GR_THREADS, 0, 0, margs, st, "expected G moments prefix");
+    if (rc) return rc;
     root_sum_kernel<<<root_grid, GR_THREADS, 0, st>>>(g, m.dist, m.sqn, mo->sq);
     GG_CHECK(cudaGetLastError());
     GG_CHECK(cudaMemsetAsync(m.pf, 0, rn * sizeof(double), st));             // Pf is spent: the plane of mn's terms

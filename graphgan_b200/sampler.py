@@ -371,14 +371,9 @@ class WalkSampler:
             return
         assert emb.dtype == torch.float32 and emb.is_contiguous() and bias.dtype == torch.float32
         reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
-        budget = int(max_scratch_bytes if max_scratch_bytes is not None else os.environ.get("GG_GDIST_SCRATCH", 2 << 30))
-
-        def scratch_bytes(k):
-            nb = C.c_int64(0)
-            _cabi.check(self.lib.gg_generator_dist_scratch_bytes(N, nnz, k, C.byref(nb)), "gg_generator_dist_scratch_bytes")
-            return nb.value
+        scratch_bytes = lambda k: self._scratch_size("gg_generator_dist_scratch_bytes", N, nnz, k)
         per_root = scratch_bytes(1) + (extra_bytes(1) if extra_bytes is not None else 0)
-        chunk = max(1, min(R, budget // max(per_root, 1), ((1 << 31) - 1) // max(N, 1)))
+        chunk = self._chunk_size(R, N, per_root, max_scratch_bytes)
         scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
         if dist is None:
             dist = torch.empty((chunk, N), dtype=torch.float64, device=self.device)
@@ -428,10 +423,9 @@ class WalkSampler:
         ok = torch.zeros(R, dtype=torch.int32, device=self.device)
         st, scratch = self._stream(), None
         for lo, hi, dist, root_ok in self._distribution_chunks(g_emb, g_bias, trees, reuse, max_scratch_bytes, None):
-            nb = C.c_int64(0)
-            _cabi.check(self.lib.gg_game_value_scratch_bytes(N, hi - lo, C.byref(nb)), "gg_game_value_scratch_bytes")
-            if scratch is None or scratch.numel() < nb.value:
-                scratch = torch.empty(max(nb.value, 16), dtype=torch.uint8, device=self.device)
+            nb = self._scratch_size("gg_game_value_scratch_bytes", N, hi - lo)
+            if scratch is None or scratch.numel() < nb:
+                scratch = torch.empty(max(nb, 16), dtype=torch.uint8, device=self.device)
             _cabi.check(self.lib.gg_game_value(N, int(d_emb.shape[1]), ptr(d_emb), ptr(d_bias), ptr(g.raw_indptr),
                                                ptr(g.raw_adj), hi - lo, ptr(trees.roots[lo:hi]), ptr(dist), ptr(root_ok),
                                                ptr(pos[lo:hi]), ptr(neg[lo:hi]), ptr(ok[lo:hi]), ptr(scratch),
@@ -460,16 +454,10 @@ class WalkSampler:
         grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
         if R == 0:
             return pos, neg, ok, grad_emb, grad_bias
-        order = torch.argsort(trees.roots.long(), stable=True)
-        st_trees = trees.select(order)
+        order, st_trees = self._by_root_id(trees)
         reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
-        budget = int(max_scratch_bytes if max_scratch_bytes is not None else os.environ.get("GG_GDIST_SCRATCH", 2 << 30))
-
-        def scratch_bytes(k):
-            nb = C.c_int64(0)
-            _cabi.check(self.lib.gg_game_value_grad_scratch_bytes(N, nnz, k, C.byref(nb)), "gg_game_value_grad_scratch_bytes")
-            return nb.value
-        chunk = max(1, min(R, budget // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        scratch_bytes = lambda k: self._scratch_size("gg_game_value_grad_scratch_bytes", N, nnz, k)
+        chunk = self._chunk_size(R, N, scratch_bytes(1), max_scratch_bytes)
         scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
         sp, sn, so = (torch.zeros_like(x) for x in (pos, neg, ok))
         d = self._law_desc(g_emb, g_bias, st_trees, reuse, None)
@@ -490,6 +478,25 @@ class WalkSampler:
         else 2 GiB."""
         return int(max_scratch_bytes if max_scratch_bytes is not None else os.environ.get("GG_GDIST_SCRATCH", 2 << 30))
 
+    def _chunk_size(self, R, N, per_root, max_scratch_bytes):
+        """roots per chunk of the exact-game entry points: as many as the scratch budget holds at ``per_root`` bytes
+        each, at most R, and fewer than 2^31 / N (the [chunk, N] planes are indexed in int32)"""
+        return max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(per_root, 1), ((1 << 31) - 1) // max(N, 1)))
+
+    def _scratch_size(self, fn, *args):
+        """the bytes the scratch-size entry point ``fn`` (its name) gives for ``args``"""
+        nb = C.c_int64(0)
+        _cabi.check(getattr(self.lib, fn)(*args, C.byref(nb)), fn)
+        return nb.value
+
+    def _by_root_id(self, trees):
+        """(order, sorted trees): the rows of ``trees`` in ascending root id order (stable for duplicates), so that the
+        bits of a sum over roots do not depend on their order; the trees are not copied when already sorted"""
+        torch = self.torch
+        R = int(trees.roots.shape[0])
+        order = torch.argsort(trees.roots.long(), stable=True)
+        return order, trees if bool(torch.equal(order, torch.arange(R, device=order.device))) else trees.select(order)
+
     def _given_law_chunks(self, law, order, max_scratch_bytes, extra_bytes):
         """The chunks of ``_distribution_chunks`` for a law computed earlier: ``law = (dist [R, N], root_ok [R])`` from
         ``distribution`` of the trees whose rows ``order`` selects.  Yields (lo, hi, dist rows, root_ok rows) of the roots
@@ -504,7 +511,7 @@ class WalkSampler:
                              % (R, N, R))
         ident = bool(torch.equal(order, torch.arange(R, device=order.device)))
         per_root = extra_bytes(1) + (0 if ident else 8 * N)
-        chunk = max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(per_root, 1), ((1 << 31) - 1) // max(N, 1)))
+        chunk = self._chunk_size(R, N, per_root, max_scratch_bytes)
         for lo in range(0, R, chunk):
             hi = min(R, lo + chunk)
             if ident:
@@ -538,19 +545,9 @@ class WalkSampler:
         grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
         if R == 0:
             return pos, neg, ok, grad_emb, grad_bias
-        order = torch.argsort(trees.roots.long(), stable=True)
-        st_trees = trees.select(order)
-
-        def value_bytes(k):
-            nb = C.c_int64(0)
-            _cabi.check(self.lib.gg_game_value_scratch_bytes(N, k, C.byref(nb)), "gg_game_value_scratch_bytes")
-            return nb.value
-
-        def grad_bytes(k):
-            nb = C.c_int64(0)
-            _cabi.check(self.lib.gg_game_value_grad_d_scratch_bytes(N, ld, k, C.byref(nb)),
-                        "gg_game_value_grad_d_scratch_bytes")
-            return nb.value
+        order, st_trees = self._by_root_id(trees)
+        value_bytes = lambda k: self._scratch_size("gg_game_value_scratch_bytes", N, k)
+        grad_bytes = lambda k: self._scratch_size("gg_game_value_grad_d_scratch_bytes", N, ld, k)
         sp, sn, so = (torch.zeros_like(x) for x in (pos, neg, ok))
         st, vs, ds = self._stream(), None, None
         extra = lambda k: value_bytes(k) + grad_bytes(k)
@@ -619,17 +616,11 @@ class WalkSampler:
         grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
         if R == 0:
             return n_pairs, ok, sq, mn, grad_emb, grad_bias, sq_node
-        order = torch.argsort(trees.roots.long(), stable=True)
-        st_trees = trees.select(order)
+        order, st_trees = self._by_root_id(trees)
         reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
         name = "gg_expected_g_moments" if moments else "gg_expected_g_grad"
-        size_fn = getattr(self.lib, name + "_scratch_bytes")
-
-        def scratch_bytes(k):
-            nb = C.c_int64(0)
-            _cabi.check(size_fn(N, nnz, k, window, C.byref(nb)), name + "_scratch_bytes")
-            return nb.value
-        chunk = max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        scratch_bytes = lambda k: self._scratch_size(name + "_scratch_bytes", N, nnz, k, window)
+        chunk = self._chunk_size(R, N, scratch_bytes(1), max_scratch_bytes)
         scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
         sn, so = torch.zeros_like(n_pairs), torch.zeros_like(ok)
         ssq, smn = (torch.zeros_like(sq), torch.zeros_like(mn)) if moments else (None, None)
@@ -680,13 +671,8 @@ class WalkSampler:
         grad_bias = torch.zeros(N, dtype=torch.float64, device=self.device)
         if R == 0:
             return accept, p_void, torch.zeros(0, dtype=torch.int32, device=self.device), grad_emb, grad_bias
-        order = torch.argsort(trees.roots.long(), stable=True)
-        st_trees = trees.select(order)
-
-        def grad_bytes(k):
-            nb = C.c_int64(0)
-            _cabi.check(self.lib.gg_expected_d_grad_scratch_bytes(N, ld, k, C.byref(nb)), "gg_expected_d_grad_scratch_bytes")
-            return nb.value
+        order, st_trees = self._by_root_id(trees)
+        grad_bytes = lambda k: self._scratch_size("gg_expected_d_grad_scratch_bytes", N, ld, k)
         sa, sv = torch.zeros_like(accept), torch.zeros_like(p_void)
         st, ds = self._stream(), None
         for lo, hi, dist, root_ok, pv in self._distribution_chunks(g_emb, g_bias, st_trees, reuse, max_scratch_bytes, None,
@@ -708,17 +694,11 @@ class WalkSampler:
         assert g_emb.dtype == torch.float32 and g_emb.is_contiguous() and g_bias.dtype == torch.float32
         assert int(g_emb.shape[0]) == g.n_node and int(g_bias.shape[0]) == g.n_node
         R, N, nnz = int(trees.roots.shape[0]), g.n_node, int(g.adj.shape[0])
-        order = torch.argsort(trees.roots.long(), stable=True)
-        ident = bool(torch.equal(order, torch.arange(R, device=order.device)))
-        st_trees = trees if ident else trees.select(order)             # (rows of nnz / 8 bytes: no copy when sorted)
+        order, st_trees = self._by_root_id(trees)
         reuse = (self.hub_threshold > 0) if reuse is None else bool(reuse)
-        fn = self.lib.gg_best_response_grad_scratch_bytes if grad else self.lib.gg_best_response_scratch_bytes
-
-        def scratch_bytes(k):
-            nb = C.c_int64(0)
-            _cabi.check(fn(N, nnz, k, C.byref(nb)), "gg_best_response_scratch_bytes")
-            return nb.value
-        chunk = max(1, min(R, self.scratch_budget(max_scratch_bytes) // max(scratch_bytes(1), 1), ((1 << 31) - 1) // max(N, 1)))
+        fn = "gg_best_response_grad_scratch_bytes" if grad else "gg_best_response_scratch_bytes"
+        scratch_bytes = lambda k: self._scratch_size(fn, N, nnz, k)
+        chunk = self._chunk_size(R, N, scratch_bytes(1), max_scratch_bytes)
         scratch = torch.empty(max(scratch_bytes(chunk), 16), dtype=torch.uint8, device=self.device)
         return order, st_trees, chunk, scratch, self._law_desc(g_emb, g_bias, st_trees, reuse, None)
 
